@@ -28,12 +28,6 @@ if ROOT not in sys.path:
 
 UNIT = "points/s"
 NU, RHO = 0.01, 1.0
-# dram__bytes_read.sum + dram__bytes_write.sum of the hidden-layer kernels of cfg3 from the committed `ncu --set full`
-# captures of this round (profiles/r02_summary.md; one 65,536-point chunk, all five hidden->hidden layers): bytes PER POINT.
-# Equal to the plane sets the design streams (no re-reads): fwd 1 read + 10 written sets, dx 6 read + 5 written, dW 10 read.
-NCU_DRAM_BYTES_PER_POINT_CFG3 = {"fwd_gemm": (364.1e6 + 3294.9e6) / 65536, "dx_gemm": (2060.0e6 + 1635.9e6) / 65536,
-                                 "dw_gemm": 5 * (671.5e6 + 4.3e6) / 65536}  # profiles/r02c_ncu_*_details.txt (final build)
-
 # name, metric label, points per GPU, dtype
 CONFIGS = {
     1: dict(metric="collocation-points/sec PDE residual loss+grad (Laplace2D)", n=10201, dtype="f32",
@@ -57,15 +51,8 @@ _T0 = time.perf_counter()
 
 
 def log(msg: str):
-    """Progress to stderr and gpurun_out/bench_progress.log (never to stdout: stdout carries the JSON line)."""
-    line = f"[bench +{time.perf_counter() - _T0:7.1f}s] {msg}"
-    print(line, file=sys.stderr, flush=True)
-    try:
-        os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-        with open(os.path.join(ROOT, "gpurun_out", "bench_progress.log"), "a") as f:
-            f.write(line + "\n")
-    except OSError:
-        pass
+    """Progress to stderr (never to stdout: stdout carries the JSON line)."""
+    print(f"[bench +{time.perf_counter() - _T0:7.1f}s] {msg}", file=sys.stderr, flush=True)
 
 
 def flops_per_point(C: int, widths_list) -> float:
@@ -75,7 +62,7 @@ def flops_per_point(C: int, widths_list) -> float:
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -111,13 +98,8 @@ class ClockSampler:
 
 
 def measured_peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            p = json.load(f)
-        return {"bf16_tflops_sustained": p.get("bf16_tflops_sustained"), "bf16_tflops": p.get("bf16_tflops"),
-                "hbm_gbs": p.get("hbm_gbs"), "source": "MEASURED_PEAKS.json"}
-    return {"bf16_tflops_sustained": 1400.0, "bf16_tflops": 1590.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    """NVIDIA's data-sheet figures for the H100 SXM (700 W): a ceiling, not a measurement."""
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet (dense, 700 W)"}
 
 
 def measure_tf32_peak(dev):
@@ -304,6 +286,17 @@ def build_workload(cfg: int, dev, rank: int):
     return model, cst, host, labels_host, dt
 
 
+def dump_outputs(out_dir: str, losses, model):
+    """The caller-visible results of the last timed step: its per-equation losses and the parameters its Adam update
+    left.  Inputs and initial weights are seeded, so two builds run with the same arguments can be compared file by file."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in losses.items():
+        np.save(os.path.join(out_dir, f"loss_{k}.npy"), v.detach().double().cpu().numpy().reshape(-1))
+    np.save(os.path.join(out_dir, "params.npy"), model.flat.data.detach().cpu().numpy())
+
+
 # --------------------------------------------------------------------------------------------------
 def run_ours(args):
     import torch
@@ -313,7 +306,7 @@ def run_ours(args):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: the engine has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py needs an H100: the engine has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -343,7 +336,7 @@ def run_ours(args):
         widths_list = [model.net_spec().widths]
     fpp = flops_per_point(C, widths_list)
     params_init = model.engine_params().detach().clone() if plan is not None else None  # parity is checked on these too
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def make_step(lab, comm=True):
         def step(inp):
@@ -381,7 +374,7 @@ def run_ours(args):
             dist.all_reduce(ms_total, op=dist.ReduceOp.MAX)
         return float(ms_total) / steps, out
 
-    log(f"setup done: config {cfg}, C={C}, tcgen05={plan.uses_tcgen05 if plan else 'n/a'}")
+    log(f"setup done: config {cfg}, C={C}, tensor cores={plan.uses_tcgen05 if plan else 'n/a'}")
     # ---------------- device-resident timing ("value") ----------------
     dev_in = {k: v.to(dev) for k, v in host.items()}
     for _ in range(args.warmup):
@@ -395,6 +388,8 @@ def run_ours(args):
     t_wall0 = time.perf_counter()
     ms_per_step, losses = timed(step, dev_in, args.steps)
     t_wall = time.perf_counter() - t_wall0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, losses, model)
     if plan is not None:
         launches_per_step = plan.last_launches + 1  # + fused Adam
     else:  # DeepONet: every two-phase call of both sub-network plans over the timed steps, + head kernels + fused Adam
@@ -601,21 +596,17 @@ def run_ours(args):
             roofline = {"bound": "hbm", "kernel": dom, "achieved": hbm, "peak": peaks["hbm_gbs"], "unit": "GB/s",
                         "frac": hbm / peaks["hbm_gbs"] if hbm else None}
         roofline.update({
-            "traffic": (NCU_DRAM_BYTES_PER_POINT_CFG3[dom] * N / dom_launches) if cfg == 3 else None,
             "class_ms_per_step": round(dom_ms, 3), "launches_per_step": dom_launches,
             "alg_flops_per_step": classes[dom] * N,
             "hbm_gbs_design_traffic": design_bytes / (dom_ms * 1e-3) / 1e9 if dom_ms > 0 else None,
             "hbm_peak_gbs": peaks["hbm_gbs"],
             "whole_step_tflops": fpp * N / (ms_per_step * 1e-3) / 1e12,
             "class_ms": {k: round(v["ms"], 3) for k, v in prof.items()},
-            "backend": "tcgen05 (3xTF32, kind::tf32)" if on_tc else ("simt-fp64" if dt == torch.float64 else "simt-fp32"),
+            "backend": "wgmma forward + dx (3xTF32), CUDA-core dW" if on_tc else ("simt-fp64" if dt == torch.float64 else "simt-fp32"),
             "note": f"{dom}: algorithmic fp32 FLOPs of the hidden->hidden layers (C={C} jet channels) / device time of the class "
                     "measured with CUDA events around every launch on the launch stream (untimed profile pass); peak = dense tf32 "
                     "GEMM throughput measured in this run (cuBLAS 8192^3, best of 8)" +
-                    (f"; bf16 sustained peak from {peaks['source']}: {peaks['bf16_tflops_sustained']}" if on_tc else "") +
-                    "; `traffic` = dram bytes per launch of this class from the committed ncu capture (profiles/r02_summary.md), "
-                    "scaled to the points per launch, not re-measured here; hbm_gbs_design_traffic = plane sets this design "
-                    "streams for the class / its time",
+                    "; hbm_gbs_design_traffic = plane sets this design streams for the class / its time",
         })
     if roofline is None:  # DeepONet (C = 1, no input derivatives): SURVEY section 8(d) gives 408 algorithmic bytes per pair
         alg_bytes = 408.0 * N
@@ -666,6 +657,9 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", type=int, default=3, choices=[1, 2, 3, 4, 5])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (per-equation losses, float64) and the parameters it "
+                         "left (model dtype) as DIR/<name>.npy")
     ap.add_argument("--graph", default="on", choices=["on", "off"],
                     help="also time the step replayed as a CUDA graph (sub-record `cuda_graph`; the headline stays the eager step)")
     args = ap.parse_args()

@@ -1,5 +1,5 @@
 """Allen-Cahn with PirateNet — the reference's SOTA example (examples/allen_cahn/allen_cahn_piratenet.py:63-193,
-conf/allen_cahn_piratenet.yaml) on the B200-native engine: same script structure and the same ``ppsci`` calls
+conf/allen_cahn_piratenet.yaml) on the H100-native engine: same script structure and the same ``ppsci`` calls
 (PirateNet with fourier + random_weight + periods, CausalMSELoss on a freshly sampled PDE batch, supervised initial
 condition, ExponentialDecay, mtl.GradNorm); the hydra / yaml layer is the plain dict below.
 

@@ -1,5 +1,5 @@
 """Laplace2D PINN — the reference's acceptance example (examples/laplace/laplace2d.py:20-140, BASELINE configs[0]) on the
-B200-native engine.  Same script structure and the same ``ppsci`` calls; the hydra / yaml layer is replaced by the
+H100-native engine.  Same script structure and the same ``ppsci`` calls; the hydra / yaml layer is replaced by the
 plain dict below (the values of examples/laplace/conf/laplace2d.yaml).  Published result to reproduce
 (docs/zh/examples/laplace2d.md:31): MSE.u(MSE_Metric) = 0.00002.
 

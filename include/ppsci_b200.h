@@ -1,5 +1,5 @@
 /*
- * ppsci_b200.h — C-ABI of the B200-native PINN PDE-residual engine.
+ * ppsci_b200.h — C-ABI of the H100-native (sm_90a) PINN PDE-residual engine.
  *
  * The reference (PaddlePaddle/PaddleScience) has no FFI: its seam for this path is the
  * Python call  ExpressionSolver.train_forward(...)  followed by  total_loss.backward()
@@ -139,7 +139,7 @@ typedef struct ppsci_plan_spec {
   double loss_weight[PPSCI_MAX_RES];
   /* tuning */
   int32_t chunk_points; /* points per internal chunk (0 = default) */
-  int32_t backend;      /* 0 = auto, 1 = force SIMT kernels, 2 = force tcgen05 kernels */
+  int32_t backend;      /* 0 = auto, 1 = force SIMT kernels, 2 = require the wgmma tensor-core kernels */
   /* Dense first-layer operand (DeepONet branch net, ppsci/arch/deeponet.py:96-106: MLP(input_dim=num_loc)):
    * when non-zero, n_in must be 1, x_cols[0] is a row-major [n_points][n_feat] matrix (n_feat up to 4096, the
    * feat_* arrays are ignored) and no input derivatives are available (n_dir must be 0). */
@@ -292,7 +292,7 @@ int ppsci_b200_sample_uniform(int32_t dtype, uint64_t seed, uint64_t offset, int
 int ppsci_b200_plan_set_profile(ppsci_plan* plan, int32_t on);
 int ppsci_b200_plan_get_profile(ppsci_plan* plan, double* ms, int64_t* count);
 
-/* 1 if the tcgen05 (tensor-core) kernels serve this plan's hidden layers, else 0. */
+/* 1 if the wgmma tensor-core kernels serve some pass (forward, dx or dW) of this plan's layers, else 0. */
 int32_t ppsci_b200_plan_uses_tcgen05(const ppsci_plan* plan);
 
 /* Fused Adam on flat buffers — replaces paddle.optimizer.Adam.step for this path
@@ -308,7 +308,7 @@ int ppsci_b200_adam_step(int32_t dtype, void* params, const void* grads, void* e
 
 /* The same Adam update with the per-step scalars in DEVICE memory: hyper_dev[4] = {lr, 1 - beta1^t, 1 - beta2^t,
  * grad_scale}.  No argument of the launch changes from step to step, so the call can be recorded into a CUDA graph
- * together with ppsci_b200_residual_loss_fwd_bwd and replayed (the B200 counterpart of the reference's
+ * together with ppsci_b200_residual_loss_fwd_bwd and replayed (the counterpart of the reference's
  * to_static=True, ppsci/solver/solver.py:487, 907-937: one captured launch train instead of a traced program).
  * zero_grads != 0 also clears the gradient buffer it consumed (optimizer.clear_grad, ppsci/solver/train.py:178). */
 int ppsci_b200_adam_step_dev(int32_t dtype, void* params, void* grads, void* exp_avg, void* exp_avg_sq,

@@ -258,7 +258,7 @@ class DeepONet(base.Arch):
         first = x[self.u_key]
         if first.device.type != "cuda" or self.flat.device != first.device:
             raise RuntimeError(
-                "paddlescience_b200.arch.DeepONet.forward runs only on a CUDA (B200) device: the engine has no "
+                "paddlescience_b200.arch.DeepONet.forward runs only on a CUDA (H100) device: the engine has no "
                 f"CPU fallback (inputs on {first.device}, parameters on {self.flat.device})")
         _, _, b, t = self._features(x)
         bias = self.flat.data[self._bias_off: self._bias_off + 1] if self.use_bias else None

@@ -456,7 +456,7 @@ class MLP(base.Arch):
         first = x[self.input_keys[0]]
         if first.device.type != "cuda" or self.flat.device != first.device:
             raise RuntimeError(
-                "paddlescience_b200.arch.MLP.forward runs only on a CUDA (B200) device: the engine has no "
+                "paddlescience_b200.arch.MLP.forward runs only on a CUDA (H100) device: the engine has no "
                 f"CPU fallback (inputs on {first.device}, parameters on {self.flat.device})")
         plan = self._plan_values()
         cols = {k: x[k].to(self.flat.dtype) for k in self.input_keys}

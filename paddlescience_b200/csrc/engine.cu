@@ -13,10 +13,8 @@
 #include <vector>
 
 #include "kernels_simt.cuh"
-#include "kernels_tc.cuh"
-#include "kernels_tc2.cuh"
-#include "kernels_fused.cuh"
 #include "kernels_thin.cuh"
+#include "kernels_wgmma.cuh"
 #include "kernels_gate.cuh"
 
 using namespace ppsci;
@@ -56,11 +54,9 @@ struct ppsci_plan {
   int actp_stride = 0;
   int ld_hidden_max = 4;
   int chunk = 0;
-  int num_sms = 148;
-  bool use_tc = false;
-  // bit0 forward, bit1 dx, bit2 dW on the tensor cores; bit3 / bit4 / bit5: CTA-pair forward / dx / dW kernels;
-  // bit6: layer-fused forward (kernels_fused.cuh).  PPSCI_B200_TC_MASK selects subsets (debugging / cross-checks).
-  // bit7: layer-fused dx chain.  bit8: tf32 fused forward also for layers wider than 128.  bit9: fp16 fused forward also for narrow layers.
+  int num_sms = 132;
+  bool use_wg = false;  // forward, dx and dW run on the wgmma kernels where the layer shapes allow (kernels_wgmma.cuh)
+  // PPSCI_B200_TC_MASK (cross-checks): bit 0 forward, bit 1 dx, bit 2 dW of the eligible layers on the tensor cores
   int tc_mask = 255;
   // device copies of the residual program
   int* d_prog = nullptr;
@@ -108,13 +104,10 @@ static inline int round4(int x) { return (x + 3) / 4 * 4; }
 
 struct Carve {
   size_t z[PPSCI_MAX_LAYERS + 1];  // z[l] for l = 1..n_layers-1 (hidden pre-activations)
-  size_t a[PPSCI_MAX_LAYERS + 1];  // a[l] = act_jets(z[l]) stashed by the tcgen05 forward for the dW kernel
   size_t y, ybar, zbar0, zbar1;
-  size_t zb[PPSCI_MAX_LAYERS + 1];  // zb[l] = Zbar_l, one buffer per hidden layer (fused dx chain: every Zbar_l outlives the chain)
   size_t wt[PPSCI_MAX_LAYERS + 1];
   size_t loss_acc;
-  size_t tc;  // scratch of the tcgen05 backend
-  size_t w16;  // fp16 hi / lo weight images of the fused forward's layers 2.. (+ per-layer |W|max and scale words)
+  size_t wimg;  // tf32 hi / lo weight images of the layers whose forward / dx run on the wgmma kernels
   // gated plans (ModifiedMLP): gated jets G_l per hidden layer, pre-activations of embed_u / embed_v and their adjoints
   size_t gt[PPSCI_MAX_LAYERS + 1];
   size_t zu, zv, zub, zvb;
@@ -122,15 +115,50 @@ struct Carve {
   size_t total;
 };
 
-static size_t tc_scratch_bytes(const ppsci_plan* P, int64_t nc);
-static bool tc_astash_needed(const ppsci_plan* P, int l);
-static bool fused_fwd_ok(const ppsci_plan* P);
-static bool fused_dx_ok(const ppsci_plan* P);
-static bool fused_fwd16_ok(const ppsci_plan* P);
-
 // gated plans: 1 when layer 1 is an embedding layer whose stored output feeds the embed_u / embed_v layers and the
 // first gated layer (PirateNet always; ModifiedMLP with a Fourier embedding, act_first >= 0), 0 when they read the seeds
 static inline int gate_emb(const ppsci_plan_spec& s) { return (s.gated == 2 || (s.gated == 1 && s.act_first >= 0)) ? 1 : 0; }
+
+static inline int act_of_layer(const ppsci_plan_spec& s, int lin);
+// layer l's forward (dx) runs on the wgmma kernel; its weight image sits at wg_img_offset (wg_imgT_offset) of the wimg
+// region: the forward images first, then the transposed ones
+static bool wg_layer(const ppsci_plan* P, int l) {
+#ifdef PPSCI_EMUL
+  (void)P; (void)l;
+  return false;
+#else
+  return P->use_wg && (P->tc_mask & 1) && wg_fwd_ok(P->spec, l, P->J);
+#endif
+}
+static bool wg_dx_layer(const ppsci_plan* P, int l) {
+#ifdef PPSCI_EMUL
+  (void)P; (void)l;
+  return false;
+#else
+  return P->use_wg && (P->tc_mask & 2) && wg_dx_ok(P->spec, l, P->J);
+#endif
+}
+static bool wg_dw_layer(const ppsci_plan* P, int l) {
+#ifdef PPSCI_EMUL
+  (void)P; (void)l;
+  return false;
+#else
+  return P->use_wg && (P->tc_mask & 4) && wg_dw_ok(P->spec, l, P->J);
+#endif
+}
+static size_t wg_img_offset(const ppsci_plan* P, int layer) {
+  size_t off = 0;
+  for (int l = 1; l < layer; ++l)  // layer 1: a dense first layer, contraction padded to the chunk width
+    if (wg_layer(P, l))
+      off += (size_t)(l == 1 ? (P->spec.widths[0] + 31) / 32 * 32 : P->spec.widths[l - 1]) * P->spec.widths[l] * 8;
+  return off;
+}
+static size_t wg_imgT_offset(const ppsci_plan* P, int layer) {
+  size_t off = wg_img_offset(P, P->spec.n_layers + 1);
+  for (int l = 2; l < layer; ++l)
+    if (wg_dx_layer(P, l)) off += (size_t)P->spec.widths[l - 1] * P->spec.widths[l] * 8;
+  return off;
+}
 
 static void carve(const ppsci_plan* P, int64_t nc, Carve* cv) {
   const size_t es = P->spec.dtype == PPSCI_F64 ? 8 : 4;
@@ -144,15 +172,11 @@ static void carve(const ppsci_plan* P, int64_t nc, Carve* cv) {
   for (int l = 1; l < L; ++l) cv->z[l] = take((size_t)P->C * nc * P->ld[l] * es);
   cv->y = take((size_t)P->C * nc * P->ld[L] * es);
   cv->ybar = take((size_t)P->C * nc * P->ld[L] * es);
-  const bool fdx = fused_dx_ok(P);
-  cv->zbar0 = take(fdx ? 0 : (size_t)P->C * nc * P->ld_hidden_max * es);
-  cv->zbar1 = take(fdx ? 0 : (size_t)P->C * nc * P->ld_hidden_max * es);
-  for (int l = 1; l < L; ++l) cv->zb[l] = take(fdx ? (size_t)P->C * nc * P->ld[l] * es : 0);
+  cv->zbar0 = take((size_t)P->C * nc * P->ld_hidden_max * es);
+  cv->zbar1 = take((size_t)P->C * nc * P->ld_hidden_max * es);
   for (int l = 2; l <= L; ++l) cv->wt[l] = take((size_t)P->spec.widths[l] * P->spec.widths[l - 1] * es);
   cv->loss_acc = take(PPSCI_MAX_RES * sizeof(double));
-  cv->tc = take(tc_scratch_bytes(P, nc));
-  cv->w16 = take(fused_fwd16_ok(P) ? (size_t)(L - 3 > 0 ? L - 3 : 0) * P->spec.widths[1] * P->spec.widths[1] * 4 + 16 * PPSCI_MAX_LAYERS : 0);
-  for (int l = 1; l < L; ++l) cv->a[l] = take(tc_astash_needed(P, l) ? (size_t)P->C * nc * P->ld[l] * es : 0);
+  cv->wimg = take(wg_imgT_offset(P, L + 1));
   const bool gated = P->spec.gated != 0;
   for (int l = 1; l < L; ++l) cv->gt[l] = take(gated ? (size_t)P->C * nc * P->ld[l] * es : 0);
   const int emb = gate_emb(P->spec);
@@ -173,7 +197,7 @@ extern "C" const char* ppsci_b200_version(void) {
 #ifdef PPSCI_EMUL
   return "ppsci_b200 0.1 (CPU emulation build: TEST ONLY)";
 #else
-  return "ppsci_b200 0.1 (sm_100a)";
+  return "ppsci_b200 0.1 (sm_90a)";
 #endif
 }
 
@@ -203,6 +227,7 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
   } else if (s->n_feat < 1 || s->n_feat > PPSCI_MAX_FEAT) {
     return fail("plan_create: n_feat out of range");
   }
+  if (s->backend < 0 || s->backend > 2) return fail("plan_create: backend must be 0 (auto), 1 (SIMT) or 2 (tensor cores)");
   if (s->n_layers < 1 || s->n_layers > PPSCI_MAX_LAYERS) return fail("plan_create: n_layers out of range");
   if (s->widths[0] != s->n_feat) return fail("plan_create: widths[0] must equal n_feat");
   for (int l = 0; l <= s->n_layers; ++l)
@@ -216,7 +241,7 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
   if (s->n_dir < 0 || s->n_dir > PPSCI_MAX_DIR) return fail("plan_create: n_dir out of range");
   if (s->act_first == PPSCI_ACT_STAN || s->act_first == PPSCI_ACT_SWISH_B)
     return fail("plan_create: act_first cannot be an activation with a trainable parameter");
-  if ((s->act == PPSCI_ACT_STAN || s->act == PPSCI_ACT_SWISH_B) && (s->gated || s->backend == 2))
+  if ((s->act == PPSCI_ACT_STAN || s->act == PPSCI_ACT_SWISH_B) && s->gated)
     return fail("plan_create: activations with a trainable parameter (stan, swish) run on plain MLP plans, CUDA-core kernels");
   if (s->gated) {  // ModifiedMLP: the gate multiplies every hidden layer's output with the (same-width) embeddings
     if (s->n_layers < 2) return fail("plan_create: a gated network needs at least one hidden layer");
@@ -230,7 +255,6 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
       if (s->widths[l] != s->widths[emb + 1]) return fail("plan_create: a gated network needs equal hidden widths");
     if (s->gated == 2 && s->widths[1] != s->widths[2])
       return fail("plan_create: gated kind 2 adds a block's input to its output: the embedding layer needs the blocks' width");
-    if (s->backend == 2) return fail("plan_create: gated networks run on the CUDA-core kernels (backend 0 or 1)");
   }
   int C = 1, kmax = 1;
   for (int d = 0; d < s->n_dir; ++d) {
@@ -347,9 +371,9 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
   if (cudaGetDevice(&dev) == cudaSuccess && cudaGetDeviceProperties(&prop, dev) == cudaSuccess) {
     P->num_sms = prop.multiProcessorCount;
 #ifndef PPSCI_EMUL
-    if (prop.major != 10) {
+    if (prop.major != 9) {
       delete P;
-      return fail("plan_create: this library is built for sm_100a (B200) only; found compute capability " +
+      return fail("plan_create: this library is built for sm_90a (H100) only; found compute capability " +
                   std::to_string(prop.major) + "." + std::to_string(prop.minor));
     }
 #endif
@@ -357,17 +381,17 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
     delete P;
     return fail("plan_create: no CUDA device available (the engine has no CPU fallback)");
   }
-  P->use_tc = tc_plan_supported(P->spec, P->C, P->kmax) && s->backend != 1 && !s->gated &&
-              s->act != PPSCI_ACT_STAN && s->act != PPSCI_ACT_SWISH_B;
-#ifdef PPSCI_EMUL
-  if (s->act_first >= 0 && s->act_first != s->act) P->use_tc = false;  // one activation across the fused layers
-  if (s->backend != 2) P->use_tc = false;  // the emulated tensor-core kernels (1,024 OS threads per CTA pair) run on request only
-#endif
+#ifndef PPSCI_EMUL
   if (const char* m = getenv("PPSCI_B200_TC_MASK")) P->tc_mask = atoi(m);
-  if (s->backend == 2 && !P->use_tc) {
+  for (int l = 2; l <= s->n_layers && s->backend != 1; ++l)
+    if (((P->tc_mask & 1) && wg_fwd_ok(*s, l, P->J)) || ((P->tc_mask & 2) && wg_dx_ok(*s, l, P->J)) ||
+        ((P->tc_mask & 4) && wg_dw_ok(*s, l, P->J)))
+      P->use_wg = true;
+#endif
+  if (s->backend == 2 && !P->use_wg) {
     delete P;
-    return fail("plan_create: backend=2 (tcgen05) requested but the plan is not eligible "
-                "(needs f32, tanh, hidden widths in {128,256}, order<=2)");
+    return fail("plan_create: backend=2 (tensor cores) requested but the plan is not eligible (needs f32, hidden widths that "
+                "are multiples of 32 up to 256, and one of the compile-time jet layouts)");
   }
 
   auto up = [&](const void* src, size_t bytes, void** dst) -> cudaError_t {
@@ -387,11 +411,11 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
     return fail(std::string("plan_create: device upload of the residual program failed: ") + cudaGetErrorString(e));
   }
   if (s->chunk_points <= 0 && getenv("PPSCI_B200_CHUNK_POINTS") == nullptr) {
-    // default chunk: keep one call's workspace under ~40 GB of the 180 GB of HBM (cfg3 at 262,144 points: 17.6 GB)
+    // default chunk: keep one call's workspace under ~20 GB of the 80 GB of HBM
     for (;;) {
       Carve cv;
       carve(P, P->chunk, &cv);
-      if (cv.total <= (size_t)40 << 30 || P->chunk <= 16384) break;
+      if (cv.total <= (size_t)20 << 30 || P->chunk <= 16384) break;
       P->chunk /= 2;
     }
   }
@@ -433,7 +457,7 @@ extern "C" int ppsci_b200_plan_get_profile(ppsci_plan* P, double* ms, int64_t* c
 #endif
   return 0;
 }
-extern "C" int32_t ppsci_b200_plan_uses_tcgen05(const ppsci_plan* P) { return (P && P->use_tc) ? 1 : 0; }
+extern "C" int32_t ppsci_b200_plan_uses_tcgen05(const ppsci_plan* P) { return (P && P->use_wg) ? 1 : 0; }
 
 // Debug / test accessor: byte offset (from the 256-aligned workspace base) of the jet planes of
 // `layer` for a call with n_points points: layer in [1, n_layers) -> hidden pre-activations Z_l,
@@ -443,8 +467,6 @@ extern "C" int64_t ppsci_b200_plan_stash_offset(const ppsci_plan* P, int64_t n_p
   const int64_t nc = n_points < P->chunk ? n_points : P->chunk;
   Carve cv;
   carve(P, nc, &cv);
-  if (layer > 100 && layer - 100 < P->spec.n_layers) return (int64_t)cv.zb[layer - 100];   // debug: Zbar_l (fused dx chain)
-  if (layer > 200 && layer - 200 < P->spec.n_layers) return (int64_t)cv.a[layer - 200];    // debug: a-stash of layer l
   if (layer == 300) return (int64_t)cv.ybar;  // output adjoints Ybar (values_bwd_kept accepts this address: no seeding copy)
   if (layer < 1 || layer > P->spec.n_layers) return -1;
   return (int64_t)(layer < P->spec.n_layers ? cv.z[layer] : cv.y);
@@ -463,15 +485,6 @@ template <typename T>
 struct Dims {
   static constexpr int TN = sizeof(T) == 8 ? 64 : 128;
 };
-
-// bring-up instrumentation: PPSCI_B200_DEBUG_TIMELINE=<device pointer> PPSCI_B200_DEBUG_KERNEL=<0 dW | 1 fwd | 2 dx>
-static long long* debug_timeline_ptr(int which) {
-  const char* dp = getenv("PPSCI_B200_DEBUG_TIMELINE");
-  if (!dp) return nullptr;
-  const char* dk = getenv("PPSCI_B200_DEBUG_KERNEL");
-  if ((dk ? atoi(dk) : 0) != which) return nullptr;
-  return reinterpret_cast<long long*>(strtoull(dp, nullptr, 0));
-}
 
 template <typename T, int KMAX>
 static int set_attrs_once(ppsci_plan* P) {
@@ -639,8 +652,8 @@ static int run(ppsci_plan* P, const CallArgs& a) {
     ga->H = s.widths[l];
   };
   // fp32 + one of the compile-time jet layouts: vectorised thin kernels (kernels_thin.cuh)
-  const int thin_lay = tc_pick_layout(P->J, PPSCI_ACT_TANH);
-  const bool thin_vec = sizeof(T) == 4 && thin_lay != TC_LAY_DYN && getenv("PPSCI_B200_NO_THINV") == nullptr;
+  const int thin_lay = pick_layout(P->J, PPSCI_ACT_TANH);
+  const bool thin_vec = sizeof(T) == 4 && thin_lay != LAY_DYN && getenv("PPSCI_B200_NO_THINV") == nullptr;
 
   if (a.want_loss) CK(cudaMemsetAsync(loss_acc, 0, PPSCI_MAX_RES * sizeof(double), st));
   // phase 1 runs the forward exactly as a training call would (stash of everything the adjoint reads), phase 2 only the adjoint
@@ -669,41 +682,27 @@ static int run(ppsci_plan* P, const CallArgs& a) {
     }
   }
 
-  if constexpr (sizeof(T) == 4) {
-    if (P->use_tc) {
-      for (int l = 2; l <= L; ++l) {  // hidden -> hidden layers and a wide output layer
-        if (!tc_layer_ok(s, l)) continue;
-        const int K = s.widths[l - 1], N = s.widths[l];
-        const long long tot = (long long)K * N;
-        ProfScope ps_(P, CLS_MISC, st);
-        PPSCI_LAUNCH(tc::k_tc_prep_w, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st,
-                     reinterpret_cast<const float*>(params) + P->w_off[l],
-                     reinterpret_cast<float*>(ws + cv.tc + tc_img_offset(s, l)), K, N, 0);
-        P->launches++;
-      }
-      if ((P->tc_mask & 1) && tc_dense_first_ok(s)) {  // dense first layer: K rounded up to the chunk width, zero rows beyond
-        const int K = s.widths[0], N = s.widths[1];
-        float* img = reinterpret_cast<float*>(ws + cv.tc + tc_dense_img_offset(s));
-        ProfScope ps_(P, CLS_MISC, st);
-        CK(cudaMemsetAsync(img, 0, (size_t)tc_dense_kpad(s) * N * 8, st));
-        PPSCI_LAUNCH(tc::k_tc_prep_w, dim3((unsigned)(((long long)K * N + 255) / 256)), dim3(256), 0, st,
-                     reinterpret_cast<const float*>(params) + P->w_off[1], img, K, N, 0);
-        P->launches++;
-      }
-      if (do_bwd && (P->tc_mask & 2)) {
-        for (int l = 2; l <= L; ++l) {
-          if (!tc_dx_ok(s, l)) continue;
-          const int K = s.widths[l], N = s.widths[l - 1];  // gemm K = fan-out, gemm N = fan-in
-          const long long tot = (long long)K * N;
-          ProfScope ps_(P, CLS_MISC, st);
-          PPSCI_LAUNCH(tc::k_tc_prep_w, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st,
-                       reinterpret_cast<const float*>(params) + P->w_off[l],
-                       reinterpret_cast<float*>(ws + cv.tc + tc_imgT_offset(s, l)), K, N, 1);
-          P->launches++;
-        }
-      }
+#ifndef PPSCI_EMUL
+  for (int l = 1; l <= L; ++l) {  // tf32 hi / lo images of the weights of the wgmma-served layers, once per call
+    const long long tot = (long long)s.widths[l - 1] * s.widths[l];
+    if (wg_layer(P, l) && a.phase != 2) {
+      ProfScope ps_(P, CLS_MISC, st);
+      if (l == 1)  // zero rows beyond the dense first layer's contraction length
+        CK(cudaMemsetAsync(ws + cv.wimg + wg_img_offset(P, 1), 0, (size_t)wg_kpad(s.widths[0]) * s.widths[1] * 8, st));
+      PPSCI_LAUNCH(wg::k_wg_prep_w, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st,
+                   reinterpret_cast<const float*>(params) + P->w_off[l], reinterpret_cast<float*>(ws + cv.wimg + wg_img_offset(P, l)),
+                   s.widths[l - 1], s.widths[l], 0);
+      P->launches++;
+    }
+    if (wg_dx_layer(P, l) && do_bwd) {  // gemm K = fan-out, gemm N = fan-in
+      ProfScope ps_(P, CLS_MISC, st);
+      PPSCI_LAUNCH(wg::k_wg_prep_w, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st,
+                   reinterpret_cast<const float*>(params) + P->w_off[l], reinterpret_cast<float*>(ws + cv.wimg + wg_imgT_offset(P, l)),
+                   s.widths[l], s.widths[l - 1], 1);
+      P->launches++;
     }
   }
+#endif
   for (int64_t c0 = 0; c0 < a.n_points; c0 += nc_max) {
     const int64_t nc = (a.n_points - c0) < nc_max ? (a.n_points - c0) : nc_max;
     const unsigned ptiles = (unsigned)((nc + TP - 1) / TP);
@@ -768,160 +767,39 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         P->launches++;
         continue;
       }
-      if constexpr (sizeof(T) == 4) {
-        if (l == 1 && P->use_tc && (P->tc_mask & 1) && tc_dense_first_ok(s)) {
-          // dense first layer (DeepONet branch net: [N][num_loc] sensor matrix) on the tensor cores: the operand is the
-          // caller's matrix itself ("activation" = identity, values only), columns beyond K read as zero
-          tc::TcFwdArgs t;
-          memset(&t, 0, sizeof(t));
+#ifndef PPSCI_EMUL
+      if (sizeof(T) == 4 && wg_layer(P, l)) {
+        wg::WgArgs w;
+        memset(&w, 0, sizeof(w));
+        w.Kdim = s.widths[l - 1];
+        if (l == 1) {  // dense first layer: the caller's [n_points][n_feat] matrix as is, columns beyond n_feat read as zero
           const int nf = s.widths[0];
-          fill_act<float>(P, reinterpret_cast<const float*>(a.x_cols[0]) + c0 * nf, nf, nc_max, A_ACT, &t.A);
-          t.A.act = PPSCI_ACT_IDENTITY;
-          t.J = P->J;
-          t.Wimg = reinterpret_cast<const float*>(ws + cv.tc + tc_dense_img_offset(s));
-          t.Kdim = tc_dense_kpad(s);
-          t.Kvalid = nf;
-          t.Nout = s.widths[1];
-          t.bias = reinterpret_cast<const float*>(params) + P->b_off[1];
-          t.Out = reinterpret_cast<float*>(ws + (L > 1 ? cv.z[1] : cv.y));
-          t.ldo = P->ld[1];
-          t.oplane = (long long)nc_max * P->ld[1];
-          t.Np = nc;
-          t.TP = TP;
-          t.num_tiles = (int)ptiles;
-          const int smem_tc = tc::tc_fwd_smem_bytes(t.Nout);
-          const unsigned gridx = ptiles < (unsigned)P->num_sms ? ptiles : (unsigned)P->num_sms;
-          void (*kd)(tc::TcFwdArgs) = tc::k_tc_fwd<tc::SLay<0, 0, 0, 0>, -1>;
-          {
-            cudaError_t e_ = cudaFuncSetAttribute(kd, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_tc);
-            if (e_ != cudaSuccess) return fail(std::string("cudaFuncSetAttribute(k_tc_fwd dense): ") + cudaGetErrorString(e_));
-          }
-          ProfScope ps_(P, CLS_FWD, st);
-          PPSCI_KLAUNCH(kd, dim3(gridx), dim3(tc::THREADS), smem_tc, st, 1, t);
-          P->launches++;
-          continue;
+          fill_act<float>(P, reinterpret_cast<const float*>(a.x_cols[0]) + c0 * nf, nf, nc_max, A_ACT, &w.A);
+          w.A.act = PPSCI_ACT_IDENTITY;
+          w.Kdim = wg_kpad(nf);
+          w.Kvalid = nf;
+        } else {
+          fill_act<float>(P, reinterpret_cast<const float*>(ws + cv.z[l - 1]), P->ld[l - 1], nc_max, A_ACT, &w.A, l - 1);
         }
-        if (l == 2 && fused_fwd16_ok(P)) {  // fused forward, fp16 hi / lo operands after the first layer (accurate for wide layers)
-          const int H = s.widths[1], NLf = L - 2;
-          unsigned char* w16 = ws + cv.w16;
-          const size_t img_bytes = (size_t)H * H * 4;
-          unsigned* absmax = reinterpret_cast<unsigned*>(w16 + (size_t)(NLf - 1) * img_bytes);
-          float* wscale = reinterpret_cast<float*>(absmax + PPSCI_MAX_LAYERS);
-          if (c0 == 0) {  // weight scales + fp16 images once per call
-            ProfScope ps_(P, CLS_MISC, st);
-            CK(cudaMemsetAsync(absmax, 0, 2 * sizeof(unsigned) * PPSCI_MAX_LAYERS, st));
-            for (int i = 1; i < NLf; ++i) {
-              const float* Wl = reinterpret_cast<const float*>(params) + P->w_off[2 + i];
-              PPSCI_LAUNCH(tc::k_w16_absmax, dim3(64), dim3(256), 0, st, Wl, (long long)H * H, absmax + i);
-              PPSCI_LAUNCH(tc::k_w16_scale, dim3(1), dim3(1), 0, st, absmax + i, wscale + i);
-              PPSCI_LAUNCH(tc::k_tc_prep_w16, dim3((unsigned)(((long long)H * H + 255) / 256)), dim3(256), 0, st, Wl,
-                           reinterpret_cast<unsigned short*>(w16 + (size_t)(i - 1) * img_bytes), H, H, wscale + i);
-              P->launches += 3;
-            }
-          }
-          tc::FusedFwd16Args ta;
-          memset(&ta, 0, sizeof(ta));
-          tc::FusedFwdArgs& t = ta.f;
-          t.J = P->J;
-          t.act = s.act;
-          t.H = H;
-          t.n_fused = NLf;
-          t.Zin = reinterpret_cast<const float*>(ws + cv.z[1]);
-          t.ld = P->ld[1];
-          t.plane = (long long)nc_max * P->ld[1];
-          for (int i = 0; i < NLf; ++i) {
-            t.Wimg[i] = i == 0 ? reinterpret_cast<const float*>(ws + cv.tc + tc_img_offset(s, 2))
-                               : reinterpret_cast<const float*>(w16 + (size_t)(i - 1) * img_bytes);
-            t.bias[i] = reinterpret_cast<const float*>(params) + P->b_off[2 + i];
-            t.Zout[i] = reinterpret_cast<float*>(ws + cv.z[2 + i]);
-            t.Astash[i] = (do_bwd && tc_astash_needed(P, 1 + i)) ? reinterpret_cast<float*>(ws + cv.a[1 + i]) : nullptr;
-          }
-          t.Np = nc;
-          t.num_tiles = (int)ptiles;
-          t.dbg = debug_timeline_ptr(3);
-          ta.wscale = wscale;
-          const int smemf = tc::fused_fwd16_smem_bytes(H);
-          const unsigned tile_pairs = (ptiles + 1) / 2, sm_pairs = (unsigned)P->num_sms / 2;
-          const unsigned gridf = 2 * (tile_pairs < sm_pairs ? tile_pairs : sm_pairs);
-          ProfScope ps_(P, CLS_FWD, st);
-          PPSCI_FUSED_LAUNCH(k_fused_fwd16, tc_pick_layout(P->J, s.act), dim3(gridf), smemf, st, ta,
-                             return fail(std::string("cudaFuncSetAttribute(k_fused_fwd16): ") + cudaGetErrorString(e_)));
-          P->launches++;
-          l = L - 1;
-          continue;
-        }
-        if (l == 2 && fused_fwd_ok(P)) {  // every hidden -> hidden layer in ONE launch, jets stay on chip between layers
-          tc::FusedFwdArgs t;
-          memset(&t, 0, sizeof(t));
-          t.J = P->J;
-          t.act = s.act;
-          t.H = s.widths[1];
-          t.n_fused = L - 2;
-          t.Zin = reinterpret_cast<const float*>(ws + cv.z[1]);
-          t.ld = P->ld[1];
-          t.plane = (long long)nc_max * P->ld[1];
-          for (int i = 0; i < L - 2; ++i) {
-            t.Wimg[i] = reinterpret_cast<const float*>(ws + cv.tc + tc_img_offset(s, 2 + i));
-            t.bias[i] = reinterpret_cast<const float*>(params) + P->b_off[2 + i];
-            t.Zout[i] = reinterpret_cast<float*>(ws + cv.z[2 + i]);
-            t.Astash[i] = (do_bwd && tc_astash_needed(P, 1 + i)) ? reinterpret_cast<float*>(ws + cv.a[1 + i]) : nullptr;
-          }
-          t.Np = nc;
-          t.num_tiles = (int)ptiles;
-          t.dbg = debug_timeline_ptr(3);
-          const int smemf = tc::fused_fwd_smem_bytes(t.H);
-          const unsigned tile_pairs = (ptiles + 1) / 2, sm_pairs = (unsigned)P->num_sms / 2;
-          const unsigned gridf = 2 * (tile_pairs < sm_pairs ? tile_pairs : sm_pairs);
-          ProfScope ps_(P, CLS_FWD, st);
-          PPSCI_FUSED_LAUNCH(k_fused_fwd, tc_pick_layout(P->J, s.act), dim3(gridf), smemf, st, t,
-                             return fail(std::string("cudaFuncSetAttribute(k_fused_fwd): ") + cudaGetErrorString(e_)));
-          P->launches++;
-          l = L - 1;  // the loop's ++l continues with the output layer
-          continue;
-        }
+        w.J = P->J;
+        w.Wimg = reinterpret_cast<const float*>(ws + cv.wimg + wg_img_offset(P, l));
+        w.Nout = s.widths[l];
+        w.bias = reinterpret_cast<const float*>(params) + P->b_off[l];
+        w.Out = reinterpret_cast<float*>(ws + (l < L ? cv.z[l] : cv.y));  // a wide output layer writes Y
+        w.ldo = P->ld[l];
+        w.oplane = (long long)nc_max * P->ld[l];
+        w.Np = nc;
+        const unsigned wtiles = (unsigned)((nc + wg::tile_points(C) - 1) / wg::tile_points(C));
+        w.num_tiles = (int)wtiles;
+        const int smem = wg::fwd_smem_bytes(w.Nout);
+        const unsigned gridx = wtiles < (unsigned)P->num_sms ? wtiles : (unsigned)P->num_sms;
+        ProfScope ps_(P, CLS_FWD, st);
+        PPSCI_WG_LAUNCH(false, wg_layout(P->J), w.Nout, dim3(gridx), smem, st, w,
+                        return fail(std::string("cudaFuncSetAttribute(k_wg_layer): ") + cudaGetErrorString(e_)));
+        P->launches++;
+        continue;
       }
-      if constexpr (sizeof(T) == 4) {
-        if (P->use_tc && (P->tc_mask & 1) && tc_layer_ok(s, l)) {
-          tc::TcFwdArgs t;
-          memset(&t, 0, sizeof(t));
-          fill_act<float>(P, reinterpret_cast<const float*>(ws + cv.z[l - 1]), P->ld[l - 1], nc_max, A_ACT, &t.A);
-          t.J = P->J;
-          t.Wimg = reinterpret_cast<const float*>(ws + cv.tc + tc_img_offset(s, l));
-          t.Kdim = s.widths[l - 1];
-          t.Nout = s.widths[l];
-          t.bias = reinterpret_cast<const float*>(params) + P->b_off[l];
-          t.Out = reinterpret_cast<float*>(ws + (l == L ? cv.y : cv.z[l]));  // a wide output layer writes Y
-          t.ldo = P->ld[l];
-          t.oplane = (long long)nc_max * P->ld[l];
-          t.Np = nc;
-          t.TP = TP;
-          t.num_tiles = (int)ptiles;
-          t.dbg = debug_timeline_ptr(1);
-          if (do_bwd && tc_astash_needed(P, l - 1)) {
-            t.Astash = reinterpret_cast<float*>(ws + cv.a[l - 1]);
-            t.lda = P->ld[l - 1];
-            t.aplane = (long long)nc_max * P->ld[l - 1];
-          }
-          const int lay_f = tc_pick_layout(P->J, s.act);
-          if ((P->tc_mask & 8) && lay_f != TC_LAY_DYN && P->num_sms >= 2) {  // CTA pairs (cta_group::2)
-            const int smem2 = tc::tc2_smem_bytes(t.Nout);
-            const unsigned tile_pairs = (ptiles + 1) / 2, sm_pairs = (unsigned)P->num_sms / 2;
-            const unsigned gridx2 = 2 * (tile_pairs < sm_pairs ? tile_pairs : sm_pairs);
-            ProfScope ps_(P, CLS_FWD, st);
-            PPSCI_TC2_LAUNCH(k_tc2_fwd, lay_f, dim3(gridx2), smem2, st, t,
-                             return fail(std::string("cudaFuncSetAttribute(k_tc2_fwd): ") + cudaGetErrorString(e_)));
-            P->launches++;
-            continue;
-          }
-          const int smem_tc = tc::tc_fwd_smem_bytes(t.Nout);
-          const unsigned gridx = ptiles < (unsigned)P->num_sms ? ptiles : (unsigned)P->num_sms;
-          ProfScope ps_(P, CLS_FWD, st);
-          PPSCI_TC_LAUNCH(k_tc_fwd, tc_pick_layout(P->J, s.act), KMAX, dim3(gridx), smem_tc, st, t,
-                          return fail(std::string("cudaFuncSetAttribute(k_tc_fwd): ") + cudaGetErrorString(e_)));
-          P->launches++;
-          continue;
-        }
-      }
+#endif
       GemmArgs<T> g;
       memset(&g, 0, sizeof(g));
       if (l == 1) fill_first<T>(P, a.x_cols, c0, nc_max, &g.A);
@@ -1059,43 +937,9 @@ static int run(ppsci_plan* P, const CallArgs& a) {
     const T* zbar_cur = reinterpret_cast<const T*>(ws + cv.ybar);
     int zbar_ld = P->ld[L];
     int flip = 0;
-    const bool fdx = fused_dx_ok(P);
-    bool fdx_done = false;
-    // destination of Zbar_{lower}: its own buffer under the fused dx chain, the two ping-pong buffers otherwise
-    auto zbar_dst = [&](int lower) -> T* {
-      return reinterpret_cast<T*>(ws + (fdx ? cv.zb[lower] : (flip ? cv.zbar1 : cv.zbar0)));
-    };
+    // destination of Zbar_{lower}: the two ping-pong buffers
+    auto zbar_dst = [&](int) -> T* { return reinterpret_cast<T*>(ws + (flip ? cv.zbar1 : cv.zbar0)); };
     for (int l = L; l >= 1; --l) {
-      if constexpr (sizeof(T) == 4) {
-        if (fdx && l == L - 1 && !fdx_done) {  // Zbar_{L-1} is in place: Zbar_{L-2} .. Zbar_1 in ONE launch
-          tc::FusedDxArgs t;
-          memset(&t, 0, sizeof(t));
-          t.J = P->J;
-          t.act = s.act;
-          t.H = s.widths[1];
-          t.n_fused = L - 2;
-          t.ZbarIn = reinterpret_cast<const float*>(ws + cv.zb[L - 1]);
-          t.ld = P->ld[1];
-          t.plane = (long long)nc_max * P->ld[1];
-          for (int i = 0; i < L - 2; ++i) {
-            const int ll = L - 1 - i;
-            t.WimgT[i] = reinterpret_cast<const float*>(ws + cv.tc + tc_imgT_offset(s, ll));
-            t.Zprev[i] = reinterpret_cast<const float*>(ws + cv.z[ll - 1]);
-            t.ZbarOut[i] = reinterpret_cast<float*>(ws + cv.zb[ll - 1]);
-          }
-          t.Np = nc;
-          t.num_tiles = (int)ptiles;
-          t.dbg = debug_timeline_ptr(4);
-          const int smemf = tc::fused_fwd_smem_bytes(t.H);
-          const unsigned tile_pairs = (ptiles + 1) / 2, sm_pairs = (unsigned)P->num_sms / 2;
-          const unsigned gridf = 2 * (tile_pairs < sm_pairs ? tile_pairs : sm_pairs);
-          ProfScope ps_(P, CLS_DX, st);
-          PPSCI_FUSED_LAUNCH(k_fused_dx, tc_pick_layout(P->J, s.act), dim3(gridf), smemf, st, t,
-                             return fail(std::string("cudaFuncSetAttribute(k_fused_dx): ") + cudaGetErrorString(e_)));
-          P->launches++;
-          fdx_done = true;
-        }
-      }
       if (l == L && thin_last) {  // dW_L, db_L and Zbar_{L-1} in one streaming pass
         LastArgs<T> f;
         memset(&f, 0, sizeof(f));
@@ -1169,83 +1013,49 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         P->launches++;
         break;
       }
-      bool dw_done = false;
-      if constexpr (sizeof(T) == 4) {
-        const bool dense_tc = l == 1 && P->use_tc && (P->tc_mask & 1) && (P->tc_mask & 4) && tc_dense_first_ok(s);
-        if (dense_tc || (l >= 2 && tc_astash_needed(P, l - 1))) {
-          tc::TcDwArgs t;
-          memset(&t, 0, sizeof(t));
-          if (dense_tc) {  // the operand of dW_1 is the caller's sensor matrix itself (fan-in rows beyond K are masked)
-            t.Aact = reinterpret_cast<const float*>(a.x_cols[0]) + c0 * s.widths[0];
-            t.lda = s.widths[0];
-            t.aplane = 0;
-          } else {
-            t.Aact = reinterpret_cast<const float*>(ws + cv.a[l - 1]);
-            t.lda = P->ld[l - 1];
-            t.aplane = (long long)nc_max * P->ld[l - 1];
-          }
-          t.J = P->J;
-          t.Zbar = reinterpret_cast<const float*>(zbar_cur);
-          t.ldzb = zbar_ld;
-          t.zbplane = (long long)nc_max * zbar_ld;
-          t.Kdim = s.widths[l - 1];
-          t.Nout = s.widths[l];
-          t.dW = reinterpret_cast<float*>(grads) + P->w_off[l];
-          t.Np = nc;
-          const int PTt = tc::KCH / C;
-          t.PT = PTt;
-          const int NC = tc_dw_cols_per_cta(s.widths[l]);
-          t.Nout = NC;
-          t.n0_stride = NC;
-          t.ldw = s.widths[l];
-          const long long total_chunks = (nc + PTt - 1) / PTt;
-          bool db_fused = false;
-          if ((P->tc_mask & 32) && t.Kdim % 256 == 0 && s.widths[l] % 256 == 0 && P->num_sms >= 2) {
-            // CTA pairs (cta_group::2): one pair per 256 x 256 block of dW and reduction split
-            const unsigned kt2 = (unsigned)(t.Kdim / 256), nb2 = (unsigned)(s.widths[l] / 256);
-            long long want2 = (P->num_sms / 2) / (kt2 * nb2);
-            if (want2 < 1) want2 = 1;
-            if (want2 > total_chunks) want2 = total_chunks;
-            const long long cps2 = (total_chunks + want2 - 1) / want2;
-            const unsigned splits2 = (unsigned)((total_chunks + cps2 - 1) / cps2);
-            t.chunks_per_split = (int)cps2;
-            t.dbg = debug_timeline_ptr(0);
-            t.db = reinterpret_cast<float*>(grads) + P->b_off[l];  // bias gradient fused into the Zbar producer
-            db_fused = true;
-            const int smem2 = tc::tc2_smem_bytes(256);
-            ProfScope ps_(P, CLS_DW, st);
-            PPSCI_TC2_LAUNCH_L(k_tc2_dw, tc_pick_layout(P->J, PPSCI_ACT_TANH), dim3(2 * kt2, splits2, nb2), smem2, st, t,
-                               return fail(std::string("cudaFuncSetAttribute(k_tc2_dw): ") + cudaGetErrorString(e_)));
-            P->launches++;
-          } else {
-          const unsigned kt = (unsigned)((t.Kdim + 127) / 128), nb = (unsigned)(s.widths[l] / NC);
-          long long want = P->num_sms / (kt * nb);
-          if (want < 1) want = 1;
-          if (want > total_chunks) want = total_chunks;
-          const long long cps = (total_chunks + want - 1) / want;
-          const unsigned splits = (unsigned)((total_chunks + cps - 1) / cps);
-          t.chunks_per_split = (int)cps;
-          t.dbg = debug_timeline_ptr(0);
-          const int smem_tc = tc::tc_dw_smem_bytes(NC);
-          {
-            ProfScope ps_(P, CLS_DW, st);
-            PPSCI_TC_LAUNCH_L(k_tc_dw, tc_pick_layout(P->J, PPSCI_ACT_TANH), KMAX, dim3(kt, splits, nb), smem_tc, st, t,
-                            return fail(std::string("cudaFuncSetAttribute(k_tc_dw): ") + cudaGetErrorString(e_)));
-            P->launches++;
-          }
-          }
-          if (!db_fused) {
-            ProfScope ps_(P, CLS_THIN_DW, st);
-            const int ppb = 512;
-            PPSCI_LAUNCH(tc::k_bias_grad, dim3((unsigned)((s.widths[l] + 127) / 128), (unsigned)((nc + ppb - 1) / ppb)), dim3(128), 0, st,
-                         reinterpret_cast<const float*>(zbar_cur), zbar_ld, (long long)nc, s.widths[l],
-                         reinterpret_cast<float*>(grads) + P->b_off[l], ppb);
-            P->launches++;
-          }
-          dw_done = true;
+#ifndef PPSCI_EMUL
+      if (sizeof(T) == 4 && wg_dw_layer(P, l)) {  // dW_l on the tensor cores, db_l beside it
+        wg::WgDwArgs w;
+        memset(&w, 0, sizeof(w));
+        if (l == 1) {  // dense first layer: the caller's matrix is the operand
+          fill_act<float>(P, reinterpret_cast<const float*>(a.x_cols[0]) + c0 * s.widths[0], s.widths[0], nc_max, A_ACT, &w.A);
+          w.A.act = PPSCI_ACT_IDENTITY;
+        } else {
+          fill_act<float>(P, reinterpret_cast<const float*>(ws + cv.z[l - 1]), P->ld[l - 1], nc_max, A_ACT, &w.A, l - 1);
         }
-      }
-      if (!dw_done)
+        w.J = P->J;
+        w.Zbar = reinterpret_cast<const float*>(zbar_cur);
+        w.ldzb = zbar_ld;
+        w.zbplane = (long long)nc_max * zbar_ld;
+        w.Kdim = s.widths[l - 1];
+        w.dW = reinterpret_cast<float*>(grads) + P->w_off[l];
+        w.Np = nc;
+        const int N = s.widths[l], PTw = wg::KCH / C;
+        const long long total_chunks = (nc + PTw - 1) / PTw;
+        const unsigned kt = (unsigned)((w.Kdim + wg::TM - 1) / wg::TM);
+        long long want = P->num_sms / kt;
+        if (want < 1) want = 1;
+        if (want > total_chunks) want = total_chunks;
+        const long long cps = (total_chunks + want - 1) / want;
+        w.chunks_per_split = (int)cps;
+        const unsigned splits = (unsigned)((total_chunks + cps - 1) / cps);
+        const int smem = wg::fwd_smem_bytes(N);
+        {
+          ProfScope ps_(P, CLS_DW, st);
+          PPSCI_WG_DW_LAUNCH(wg_layout(P->J), N, dim3(kt, splits), smem, st, w,
+                             return fail(std::string("cudaFuncSetAttribute(k_wg_dw): ") + cudaGetErrorString(e_)));
+          P->launches++;
+        }
+        {
+          ProfScope ps_(P, CLS_THIN_DW, st);
+          const int ppb = 512;
+          PPSCI_LAUNCH(wg::k_wg_bias_grad, dim3((unsigned)((N + 127) / 128), (unsigned)((nc + ppb - 1) / ppb)), dim3(128), 0, st,
+                       reinterpret_cast<const float*>(zbar_cur), zbar_ld, (long long)nc, N,
+                       reinterpret_cast<float*>(grads) + P->b_off[l], ppb);
+          P->launches++;
+        }
+      } else
+#endif
       {  // dW_l, db_l
         DwArgs<T> g;
         memset(&g, 0, sizeof(g));
@@ -1300,57 +1110,40 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         }
       }
       if (l == 1) break;
-      if (fdx && l <= L - 1) {  // Zbar_{l-1} was produced by the fused chain
-        zbar_cur = reinterpret_cast<const T*>(ws + cv.zb[l - 1]);
+#ifndef PPSCI_EMUL
+      if (sizeof(T) == 4 && wg_dx_layer(P, l)) {  // Zbar_{l-1} on the tensor cores
+        wg::WgArgs w;
+        memset(&w, 0, sizeof(w));
+        fill_act<float>(P, reinterpret_cast<const float*>(zbar_cur), zbar_ld, nc_max, A_PLAIN, &w.A);
+        w.J = P->J;
+        w.Wimg = reinterpret_cast<const float*>(ws + cv.wimg + wg_imgT_offset(P, l));
+        w.Kdim = s.widths[l];
+        w.Nout = s.widths[l - 1];
+        float* outp = reinterpret_cast<float*>(zbar_dst(l - 1));
+        w.Out = outp;
+        w.ldo = P->ld[l - 1];
+        w.oplane = (long long)nc_max * P->ld[l - 1];
+        w.Np = nc;
+        const unsigned wtiles = (unsigned)((nc + wg::tile_points(C) - 1) / wg::tile_points(C));
+        w.num_tiles = (int)wtiles;
+        w.Zprev = reinterpret_cast<const float*>(ws + cv.z[l - 1]);
+        w.ldz = P->ld[l - 1];
+        w.zplane = (long long)nc_max * P->ld[l - 1];
+        w.act = act_of_layer(s, l - 1);
+        const int smem = wg::fwd_smem_bytes(w.Nout);
+        const unsigned gridx = wtiles < (unsigned)P->num_sms ? wtiles : (unsigned)P->num_sms;
+        {
+          ProfScope ps_(P, CLS_DX, st);
+          PPSCI_WG_LAUNCH(true, wg_layout(P->J), w.Nout, dim3(gridx), smem, st, w,
+                          return fail(std::string("cudaFuncSetAttribute(k_wg_layer dx): ") + cudaGetErrorString(e_)));
+          P->launches++;
+        }
+        zbar_cur = reinterpret_cast<const T*>(outp);
         zbar_ld = P->ld[l - 1];
+        flip ^= 1;
         continue;
       }
-      if constexpr (sizeof(T) == 4) {
-        if (P->use_tc && (P->tc_mask & 2) && tc_dx_ok(s, l)) {
-          tc::TcDxArgs t;
-          memset(&t, 0, sizeof(t));
-          fill_act<float>(P, reinterpret_cast<const float*>(zbar_cur), zbar_ld, nc_max, A_PLAIN, &t.A);
-          t.J = P->J;
-          t.Wimg = reinterpret_cast<const float*>(ws + cv.tc + tc_imgT_offset(s, l));
-          t.Kdim = s.widths[l];
-          t.Nout = s.widths[l - 1];
-          t.Zprev = reinterpret_cast<const float*>(ws + cv.z[l - 1]);
-          t.ldz = P->ld[l - 1];
-          t.zplane = (long long)nc_max * P->ld[l - 1];
-          t.act = s.act;
-          float* outp = reinterpret_cast<float*>(zbar_dst(l - 1));
-          t.Out = outp;
-          t.ldo = P->ld[l - 1];
-          t.oplane = (long long)nc_max * P->ld[l - 1];
-          t.Np = nc;
-          t.TP = TP;
-          t.num_tiles = (int)ptiles;
-          t.dbg = debug_timeline_ptr(2);
-          const int lay_x = tc_pick_layout(P->J, s.act);
-          if ((P->tc_mask & 16) && lay_x != TC_LAY_DYN && P->num_sms >= 2) {  // CTA pairs (cta_group::2)
-            const int smem2 = tc::tc2_smem_bytes(t.Nout);
-            const unsigned tile_pairs = (ptiles + 1) / 2, sm_pairs = (unsigned)P->num_sms / 2;
-            const unsigned gridx2 = 2 * (tile_pairs < sm_pairs ? tile_pairs : sm_pairs);
-            ProfScope ps_(P, CLS_DX, st);
-            PPSCI_TC2_LAUNCH(k_tc2_dx, lay_x, dim3(gridx2), smem2, st, t,
-                             return fail(std::string("cudaFuncSetAttribute(k_tc2_dx): ") + cudaGetErrorString(e_)));
-            P->launches++;
-          } else {
-          const int smem_tc = tc::tc_fwd_smem_bytes(t.Nout);
-          const unsigned gridx = ptiles < (unsigned)P->num_sms ? ptiles : (unsigned)P->num_sms;
-          {
-            ProfScope ps_(P, CLS_DX, st);
-            PPSCI_TC_LAUNCH(k_tc_dx, tc_pick_layout(P->J, s.act), KMAX, dim3(gridx), smem_tc, st, t,
-                            return fail(std::string("cudaFuncSetAttribute(k_tc_dx): ") + cudaGetErrorString(e_)));
-            P->launches++;
-          }
-          }
-          zbar_cur = reinterpret_cast<const T*>(outp);
-          zbar_ld = P->ld[l - 1];
-          flip ^= 1;
-          continue;
-        }
-      }
+#endif
       {  // Zbar_{l-1}
         GemmArgs<T> g;
         memset(&g, 0, sizeof(g));
@@ -1559,7 +1352,7 @@ extern "C" int ppsci_b200_deeponet_head(int32_t dtype, int32_t act, const void* 
   if ((bbar == nullptr) != (tbar == nullptr)) return fail("deeponet_head: bbar and tbar must both be given or both be null");
   if (act < 0 || act > PPSCI_ACT_LAST) return fail("deeponet_head: unknown activation");
   if (act_has_param(act)) return fail("deeponet_head: activations with a trainable parameter are not offered here");
-  const long long warps = n < 148LL * 64 ? n : 148LL * 64;  // 8 warps per block
+  const long long warps = n < 132LL * 64 ? n : 132LL * 64;  // 8 warps per block
   const unsigned blocks = (unsigned)((warps + 7) / 8);
   if (dtype == PPSCI_F64) {
     auto k = k_deeponet_head<double>;
@@ -1646,62 +1439,4 @@ extern "C" int ppsci_b200_adam_step_dev(int32_t dtype, void* params, void* grads
   }
   CK(cudaGetLastError());
   return 0;
-}
-
-// a_l is stashed by the tensor-core forward of layer l+1 and consumed by the tensor-core dW of layer l+1
-static bool tc_astash_needed(const ppsci_plan* P, int l) {
-  const int lay = l + 1;
-  return P->use_tc && (P->tc_mask & 1) && (P->tc_mask & 4) && lay <= P->spec.n_layers && tc_layer_ok(P->spec, lay) &&
-         tc_dw_ok(P->spec, lay);
-}
-static size_t tc_scratch_bytes(const ppsci_plan* P, int64_t nc) {
-  return P->use_tc ? tc_scratch_bytes_impl(P->spec, P->C, nc) : 0;
-}
-
-// layer-fused forward: fp32 tanh, one of the static jet layouts, at least one hidden -> hidden layer, all hidden
-// widths equal (K = N = H, a multiple of 32 up to 256)
-static bool fused_fwd_ok(const ppsci_plan* P) {
-  const ppsci_plan_spec& s = P->spec;
-  const int L = s.n_layers;
-  if (!P->use_tc || !(P->tc_mask & 1) || !(P->tc_mask & 8) || !(P->tc_mask & 64) || P->num_sms < 2) return false;
-  if (L < 3 || L - 2 > tc::FUSE_MAXL) return false;
-  if (tc_pick_layout(P->J, s.act) == TC_LAY_DYN) return false;
-  for (int l = 2; l < L; ++l)
-    if (!tc_layer_ok(s, l) || s.widths[l] != s.widths[1]) return false;
-  // Accuracy gate.  The fused forward double-buffers ONE accumulator per layer (2 x 256 TMEM columns), i.e. all 12
-  // round-toward-zero accumulations of a 32-wide chunk land in the big accumulator: measured on cfg3 (6 x 256) the
-  // residual error is 1.3e-5 against 4.4e-6 for the layer-at-a-time kernels, whose exact-product | cross-term split
-  // needs all 512 columns.  Up to 128-wide layers the contraction is short enough (cfg2: 1.8e-6) and the fused kernel is
-  // the default; wider layers take it only on request (PPSCI_B200_TC_MASK bit 8).  The dx chain has no such gate: its
-  // rounding only enters the weight gradient (cfg3: 1.1e-5 against a 5e-5 tolerance).
-  if (s.widths[1] > 128 && !(P->tc_mask & 256)) return false;
-  return s.widths[1] <= 256;
-}
-
-// layer-fused dx chain: same shape constraints as the fused forward, dx of every hidden -> hidden layer tensor-core eligible
-static bool fused_dx_ok(const ppsci_plan* P) {
-  const ppsci_plan_spec& s = P->spec;
-  const int L = s.n_layers;
-  if (!P->use_tc || !(P->tc_mask & 2) || !(P->tc_mask & 16) || !(P->tc_mask & 128) || P->num_sms < 2) return false;
-  if (L < 3 || L - 2 > tc::FUSE_MAXL) return false;
-  if (tc_pick_layout(P->J, s.act) == TC_LAY_DYN) return false;
-  for (int l = 2; l < L; ++l)
-    if (!tc_dx_ok(s, l) || s.widths[l] != s.widths[1]) return false;
-  return s.widths[1] <= 256;
-}
-
-// fp16-operand fused forward (k_fused_fwd16): the shape constraints of the fused forward, width a multiple of 64, at
-// least two fused layers; the default for layers wider than 128 (where the single tf32 accumulator is not accurate
-// enough), on request (PPSCI_B200_TC_MASK bit 9) for narrower ones
-static bool fused_fwd16_ok(const ppsci_plan* P) {
-  const ppsci_plan_spec& s = P->spec;
-  const int L = s.n_layers;
-  if (!P->use_tc || !(P->tc_mask & 1) || !(P->tc_mask & 8) || !(P->tc_mask & 64) || P->num_sms < 2) return false;
-  if (L < 4 || L - 2 > tc::FUSE_MAXL) return false;
-  if (tc_pick_layout(P->J, s.act) == TC_LAY_DYN || s.act != PPSCI_ACT_TANH) return false;
-  for (int l = 2; l < L; ++l)
-    if (!tc_layer_ok(s, l) || s.widths[l] != s.widths[1]) return false;
-  if (s.widths[1] % 64 != 0 || s.widths[1] > 256) return false;
-  if (P->tc_mask & 256) return false;  // bit 8: force the tf32 fused forward (cross-check)
-  return s.widths[1] > 128 || (P->tc_mask & 512);
 }

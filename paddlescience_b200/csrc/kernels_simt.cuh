@@ -1,6 +1,6 @@
 // kernels_simt.cuh — generic (any width / activation / order<=4 / f32|f64) CUDA-core kernels
-// of the jet engine.  They are the correctness anchor and the cross-check for the tcgen05
-// kernels (kernels_tc.cuh) that take over the wide fp32 tanh layers.
+// of the jet engine: every hidden layer runs on them, and they are the correctness anchor for the
+// vectorised fp32 thin-layer kernels (kernels_thin.cuh).
 //
 // Data layout (all in the caller's workspace; see DESIGN.md "HBM layout"):
 //   jets of a layer are CHANNEL-MAJOR planes   Z[c][p][h] ,  c < C, p < Np, h < ld

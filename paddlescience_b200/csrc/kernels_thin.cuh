@@ -3,21 +3,21 @@
 // The input layer (K = n_feat = 2..8) and the output layer (N = n_out = 1..8) are pure HBM streams: one pass
 // over a [C][Np][width] jet plane set.  The generic kernels in kernels_simt.cuh keep the channel structure at run
 // time (channel-indexed accumulators end up in local memory) and move 4 bytes per thread and instruction; these
-// specialisations fix the layout at compile time (tc::SLay), move 16 bytes per thread and instruction along the
+// specialisations fix the layout at compile time (SLay, jet_layout.cuh), move 16 bytes per thread and instruction along the
 // hidden dimension, and evaluate the input seeds once per point into shared memory instead of once per thread.
 // Same arithmetic (jet_math.h); the generic kernels remain the fallback (fp64, runtime layouts, odd widths) and
 // the on-GPU cross-check (PPSCI_B200_NO_THINV=1).
 #pragma once
-#include "kernels_tc.cuh"
+#include "jet_layout.cuh"
 
 namespace ppsci {
 namespace thin {
 
 constexpr int PB = 32;  // points per seed tile
-using Lay22 = tc::SLay<2, 2, 0, 0>;
-using Lay12 = tc::SLay<1, 2, 0, 0>;
-using Lay222 = tc::SLay<2, 2, 2, 0>;
-using LayV = tc::SLay<0, 0, 0, 0>;
+using Lay22 = SLay<2, 2, 0, 0>;
+using Lay12 = SLay<1, 2, 0, 0>;
+using Lay222 = SLay<2, 2, 2, 0>;
+using LayV = SLay<0, 0, 0, 0>;
 
 __device__ __forceinline__ float f4c(const float4& v, int t) { return t == 0 ? v.x : t == 1 ? v.y : t == 2 ? v.z : v.w; }
 
@@ -307,12 +307,12 @@ __global__ void __launch_bounds__(256) k_last_bwd_v(LastArgs<float> g) {
 
 }  // namespace thin
 
-// layout x (n_out for the last-layer kernels) dispatch; `lay` from tc_pick_layout(J, PPSCI_ACT_TANH), never TC_LAY_DYN
+// layout x (n_out for the last-layer kernels) dispatch; `lay` from pick_layout(J, PPSCI_ACT_TANH), never LAY_DYN
 #define PPSCI_THIN_PICK_L(KERNEL, lay, kmax, kfn)                                                  \
   switch (lay) {                                                                                   \
-    case TC_LAY_22: kfn = thin::KERNEL<thin::Lay22, kmax>; break;                                  \
-    case TC_LAY_12: kfn = thin::KERNEL<thin::Lay12, kmax>; break;                                  \
-    case TC_LAY_222: kfn = thin::KERNEL<thin::Lay222, kmax>; break;                                \
+    case LAY_22: kfn = thin::KERNEL<thin::Lay22, kmax>; break;                                  \
+    case LAY_12: kfn = thin::KERNEL<thin::Lay12, kmax>; break;                                  \
+    case LAY_222: kfn = thin::KERNEL<thin::Lay222, kmax>; break;                                \
     default: kfn = thin::KERNEL<thin::LayV, kmax>;                                                 \
   }
 #define PPSCI_THIN_PICK_LM_(KERNEL, LAY, m, kfn)                                                   \
@@ -324,9 +324,9 @@ __global__ void __launch_bounds__(256) k_last_bwd_v(LastArgs<float> g) {
   }
 #define PPSCI_THIN_PICK_LM(KERNEL, lay, m, kfn)                                                    \
   switch (lay) {                                                                                   \
-    case TC_LAY_22: PPSCI_THIN_PICK_LM_(KERNEL, thin::Lay22, m, kfn); break;                       \
-    case TC_LAY_12: PPSCI_THIN_PICK_LM_(KERNEL, thin::Lay12, m, kfn); break;                       \
-    case TC_LAY_222: PPSCI_THIN_PICK_LM_(KERNEL, thin::Lay222, m, kfn); break;                     \
+    case LAY_22: PPSCI_THIN_PICK_LM_(KERNEL, thin::Lay22, m, kfn); break;                       \
+    case LAY_12: PPSCI_THIN_PICK_LM_(KERNEL, thin::Lay12, m, kfn); break;                       \
+    case LAY_222: PPSCI_THIN_PICK_LM_(KERNEL, thin::Lay222, m, kfn); break;                     \
     default: PPSCI_THIN_PICK_LM_(KERNEL, thin::LayV, m, kfn);                                      \
   }
 

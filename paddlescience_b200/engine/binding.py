@@ -1,8 +1,8 @@
 """ctypes binding of the C-ABI declared in ``include/ppsci_b200.h``.
 
-The product path loads ``paddlescience_b200/lib/libppsci_b200.so`` (hand-written sm_100a CUDA,
+The product path loads ``paddlescience_b200/lib/libppsci_b200.so`` (hand-written sm_90a CUDA,
 built in-tree by ``paddlescience_b200.engine.build``).  There is NO CPU fallback: if the
-library is missing or no B200 is visible, every compute entry point raises.
+library is missing or no H100 is visible, every compute entry point raises.
 """
 from __future__ import annotations
 

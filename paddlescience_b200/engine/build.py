@@ -1,4 +1,4 @@
-"""In-tree build of the native library (hand-written CUDA for sm_100a, C-ABI in include/)."""
+"""In-tree build of the native library (hand-written CUDA for sm_90a, C-ABI in include/)."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ SRC = os.path.join(PKG, "csrc")
 OUT = os.path.join(PKG, "lib", "libppsci_b200.so")
 
 NVCC_FLAGS = [
-    "-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 
@@ -28,18 +28,14 @@ def sources():
     return sorted(os.path.join(SRC, f) for f in os.listdir(SRC))
 
 
-def build_native(force: bool = False, verbose: bool = False, timeline: bool = False) -> str:
-    """``timeline=True`` builds the bring-up variant ``libppsci_b200_timeline.so`` (-DPPSCI_B200_TIMELINE: clock64 stamps
-    in the tensor-core kernels, used by tests/tools/timeline*.py); the product library carries no stamp code."""
-    out = OUT.replace("libppsci_b200.so", "libppsci_b200_timeline.so") if timeline else OUT
+def build_native(force: bool = False, verbose: bool = False) -> str:
+    out = OUT
     deps = sources() + [os.path.join(ROOT, "include", "ppsci_b200.h")]
     if not force and os.path.exists(out) and all(os.path.getmtime(out) >= os.path.getmtime(d) for d in deps):
         return out
     os.makedirs(os.path.dirname(out), exist_ok=True)
     cmd = [_nvcc()] + NVCC_FLAGS + ["-I" + os.path.join(ROOT, "include"), "-I" + SRC,
                                     os.path.join(SRC, "engine.cu"), "-o", out]
-    if timeline:
-        cmd.insert(1, "-DPPSCI_B200_TIMELINE")
     if verbose:
         cmd.insert(1, "-Xptxas=-v")
     subprocess.run(cmd, check=True)

@@ -1,6 +1,6 @@
 """Residual compiler: sympy expressions -> (jet directions, register program).
 
-This is the B200-native counterpart of ``ppsci.lambdify`` (reference:
+This is the H100-native counterpart of ``ppsci.lambdify`` (reference:
 ppsci/utils/symbolic.py:681-981).  The reference turns a sympy tree into a list of
 ``nn.Layer`` nodes whose ``DerivativeNode``s call reverse-mode ``paddle.grad``
 (symbolic.py:270-403).  Here the same tree is compiled ONCE into

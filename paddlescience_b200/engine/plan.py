@@ -122,7 +122,7 @@ class ResidualPlan:
         s.grad_reg = C.cast(self._greg, C.POINTER(C.c_int32))
         s.chunk_points = int(chunk_points)
         if int(backend) == 0 and os.environ.get("PPSCI_B200_BACKEND"):
-            backend = int(os.environ["PPSCI_B200_BACKEND"])  # 1 = force SIMT kernels, 2 = force tcgen05
+            backend = int(os.environ["PPSCI_B200_BACKEND"])  # 1 = force SIMT kernels, 2 = require the wgmma kernels
         s.backend = int(backend)
         self.spec = s
         handle = C.c_void_p()

@@ -109,7 +109,7 @@ class FlatAdam:
         if p.grad is None:
             return
         if p.device.type != "cuda":
-            raise RuntimeError("FlatAdam.step needs parameters on a CUDA (B200) device: no CPU fallback")
+            raise RuntimeError("FlatAdam.step needs parameters on a CUDA (H100) device: no CPU fallback")
         self._ensure_state()
         self.t += 1
         self._clip()
@@ -166,7 +166,7 @@ class FlatAdam:
             raise NotImplementedError("CUDA-graph replay (to_static) with learnable equation parameters is not supported yet")
         p = self.model.flat
         if p.device.type != "cuda":
-            raise RuntimeError("FlatAdam.step_dev needs parameters on a CUDA (B200) device: no CPU fallback")
+            raise RuntimeError("FlatAdam.step_dev needs parameters on a CUDA (H100) device: no CPU fallback")
         if hyper_dev.dtype != torch.float64 or hyper_dev.numel() < 4 or hyper_dev.device != p.device:
             raise ValueError("hyper_dev must be a float64 tensor of 4 values on the parameters' device")
         self._ensure_state()
@@ -276,7 +276,7 @@ class FlatLBFGS:
 
     def step(self, closure):
         if self.model.flat.device.type != "cuda":
-            raise RuntimeError("FlatLBFGS.step needs parameters on a CUDA (B200) device: no CPU fallback")
+            raise RuntimeError("FlatLBFGS.step needs parameters on a CUDA (H100) device: no CPU fallback")
         if callable(self._lr):
             self.set_lr(self._lr())
         return self._opt.step(closure)

@@ -1,7 +1,7 @@
 """One training iteration recorded as a CUDA graph and replayed (``Solver(to_static=True)``).
 
 The reference's ``to_static=True`` (ppsci/solver/solver.py:487, 907-937) hands the forward to a tracing compiler so that
-small problems stop paying the per-operator host overhead.  On B200 the same goal needs no compiler: the iteration is
+small problems stop paying the per-operator host overhead.  On the H100 the same goal needs no compiler: the iteration is
 already a fixed launch train (input packing, the fused residual / adjoint kernels behind
 ``ppsci_b200_residual_loss_fwd_bwd``, loss aggregation, ``ppsci_b200_adam_step_dev``), so it is captured once per batch
 signature and replayed with one ``cudaGraphLaunch`` per step.  Everything that changes from step to step lives in device

@@ -1,5 +1,5 @@
 """``Solver`` — orchestration with the reference's constructor and public methods
-(ppsci/solver/solver.py:62-1116), hosting the B200-native hot loop.
+(ppsci/solver/solver.py:62-1116), hosting the H100-native hot loop.
 
 Kept: ``Solver(model, constraint, output_dir, optimizer, lr_scheduler, epochs, iters_per_epoch,
 update_freq, save_freq, log_freq, ..., equation, geom, validator, ...)``, ``train()``, ``eval()``,
@@ -140,7 +140,7 @@ class Solver:
     # ------------------------------------------------------------------------------------------
     def train(self):
         if self.device.type != "cuda":
-            raise RuntimeError("Solver.train needs a CUDA (B200) device: the engine has no CPU fallback")
+            raise RuntimeError("Solver.train needs a CUDA (H100) device: the engine has no CPU fallback")
         if self.optimizer is None:
             raise ValueError("Solver.train needs an optimizer")
         start_epoch = self.best_metric["epoch"] + 1
@@ -175,7 +175,7 @@ class Solver:
                 no_grad: bool = True, return_numpy: bool = False):
         """Batched forward of the model (+ expressions) — solver.py:729-872 without the DP gather."""
         if self.device.type != "cuda":
-            raise RuntimeError("Solver.predict needs a CUDA (B200) device: the engine has no CPU fallback")
+            raise RuntimeError("Solver.predict needs a CUDA (H100) device: the engine has no CPU fallback")
         n = len(next(iter(input_dict.values())))
         bs = n if batch_size is None else batch_size
         chunks: Dict[str, list] = {}

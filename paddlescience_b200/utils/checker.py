@@ -1,6 +1,6 @@
 """``ppsci.utils.run_check`` (reference: ppsci/utils/checker.py:34-117): a two-epoch Navier-Stokes smoke training plus
 one evaluation through the public API — here it exercises the native library end to end (fused residual / loss / weight-
-gradient call, fused Adam, forward-only evaluation).  Needs a B200: the engine has no CPU fallback."""
+gradient call, fused Adam, forward-only evaluation).  Needs an H100: the engine has no CPU fallback."""
 from __future__ import annotations
 
 import traceback
@@ -40,8 +40,8 @@ def run_check() -> bool:
         solver.eval(epochs)
     except Exception as e:  # noqa: BLE001 — the reference reports any failure the same way
         traceback.print_exc()
-        logger.error(f"the B200-native ppsci engine meets some problem with \n {repr(e)} \nplease check that the native "
-                     "library is built (python -c 'import __graft_entry__ as g; g.build()') and a B200 is visible.")
+        logger.error(f"the H100-native ppsci engine meets some problem with \n {repr(e)} \nplease check that the native "
+                     "library is built (python -c 'import __graft_entry__ as g; g.build()') and an H100 is visible.")
         return False
-    logger.message("ppsci (B200-native engine) is installed successfully.")
+    logger.message("ppsci (H100-native engine) is installed successfully.")
     return True

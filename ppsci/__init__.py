@@ -1,4 +1,4 @@
-"""Import shim: ``import ppsci`` resolves to the B200-native implementation so that scripts
+"""Import shim: ``import ppsci`` resolves to the H100-native implementation so that scripts
 written against PaddleScience's hot-path API run unchanged (see INTEGRATION.md)."""
 import sys as _sys
 

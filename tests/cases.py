@@ -1,4 +1,4 @@
-"""Shared parity cases: engine (CUDA library on a B200, or the CPU emulation build of the same
+"""Shared parity cases: engine (CUDA library on an H100, or the CPU emulation build of the same
 kernel sources) versus the torch oracle (oracle/ppsci_oracle.py), same seeded inputs."""
 from __future__ import annotations
 
@@ -128,7 +128,7 @@ LATE_CASES = {
                              exprs=lambda: O.laplace_expr(2), dtype=torch.float32),
 }
 
-# shapes served by the tcgen05 kernels (hidden widths multiple of 32/128); CPU emulation skips them
+# wide fp32 shapes (too slow for the CPU emulation, which skips them)
 TC_CASES = {
     "ns_f32_tc_256": dict(in_keys=("x", "y"), out_keys=("u", "v", "p"), hidden=[256, 256, 256], act="tanh",
                           exprs=lambda: O.navier_stokes_expr(0.01, 1.0, 2, False), dtype=torch.float32),
@@ -141,13 +141,13 @@ TC_CASES = {
     "ns_f32_tc_256_chunks": dict(in_keys=("x", "y"), out_keys=("u", "v", "p"), hidden=[256, 256, 256], act="tanh",
                                  exprs=lambda: O.navier_stokes_expr(0.01, 1.0, 2, False), dtype=torch.float32,
                                  chunk_div=3, weights=True),
-    # widths that give odd K-chunk counts (3, 5), odd 32-column block counts and a 16-row weight half per CTA
+    # widths that give odd K-chunk counts (3, 5) and odd 32-column block counts (an m64n32 block beside the m64n64 ones)
     "ns_f32_tc_mixed": dict(in_keys=("x", "y"), out_keys=("u", "v", "p"), hidden=[96, 160, 64, 32], act="tanh",
                             exprs=lambda: O.navier_stokes_expr(0.01, 1.0, 2, False), dtype=torch.float32),
-    # C = 7 (three second-order directions): pair kernels with two producer groups of 5 warps + 4 idle producer warps
+    # C = 7 (three second-order directions): 9 points per 64-row tile, 63 rows used
     "ns3d_f32_tc_256": dict(in_keys=("x", "y", "z"), out_keys=("u", "v", "w", "p"), hidden=[256, 256, 256], act="tanh",
                             exprs=lambda: O.navier_stokes_expr(0.05, 1.0, 3, False), dtype=torch.float32),
-    # C = 1 (no derivatives: a boundary / supervised constraint): 128 points per tile, three producer passes
+    # C = 1 (no derivatives: a boundary / supervised constraint): 64 points per tile, two producer passes
     "value_f32_tc_256": dict(in_keys=("x", "y"), out_keys=("u", "v"), hidden=[256, 256, 256], act="tanh",
                              exprs=lambda: _value_exprs(), dtype=torch.float32, labels_rand=True),
     "biharmonic_f32_tc_128": dict(in_keys=("x", "y"), out_keys=("u",), hidden=[128, 128, 128], act="tanh",

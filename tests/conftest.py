@@ -9,4 +9,4 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: test needs a real H100 (run with -m gpu)")

@@ -5,20 +5,6 @@
 // concurrently.  It exists so that indexing / tiling / barrier-protocol / descriptor logic can be checked against the
 // oracle on a box without a GPU.  It is never linked into the product library and the package never loads it
 // (tests/emul/build_emul.py builds tests/emul/_build/libppsci_b200_emul.so, loaded only by tests/).
-//
-// Round 2: the tcgen05 / TMEM / mbarrier / bulk-copy / cluster primitives the tensor-core kernels are written against
-// are emulated too (tests/emul/tc_emul_prims.h maps the PTX wrappers of kernels_tc*.cuh onto the functions below):
-//   * shared memory: one arena per CTA; a "shared-window address" is the byte offset into the arena (+ SMEM_BASE),
-//   * mbarrier: phase / pending-arrival / tx-byte state per (CTA, address), blocking waits with a deadlock timeout,
-//   * TMEM: 128 lanes x 512 fp32 columns per CTA, tcgen05.ld 32x32b checks the warp's lane quadrant,
-//   * tcgen05.mma: UMMA shared-memory descriptors are DECODED (start address, SBO, 128-byte swizzle as the hardware
-//     applies it: address bits [4,7) ^= bits [7,10)), kind::tf32 operands are truncated to 10 mantissa bits, the
-//     K = 8 products of one instruction are summed exactly and the fp32 accumulate rounds toward zero (what the
-//     hardware does — see tests/microbench/tc_numerics.cu; PPSCI_EMUL_ACC_RN=1 switches to round-to-nearest).
-//     MMAs are QUEUED at issue and executed at the next tcgen05.commit of the issuing thread: the latest moment the
-//     hardware may read the operands, so a stage that is overwritten before its commit is observed shows up as wrong
-//     results here,
-//   * cta_group::2: M = 256 over the pair (128 TMEM lanes per CTA), each CTA supplies its own A rows and N/2 rows of B.
 #pragma once
 #ifndef PPSCI_EMUL
 #error "cuda_emul.h is only for -DPPSCI_EMUL builds"
@@ -91,32 +77,14 @@ struct Barrier {
   }
 };
 
-struct MBar {
-  uint32_t init_count = 0, pending = 0;
-  long long tx = 0;
-  uint32_t phase = 0;
-  bool valid = false;
-};
-
-struct MmaRec {  // one queued tcgen05.mma
-  int group;     // 1 or 2
-  int kind;      // 0 tf32, 1 f16, 2 bf16
-  uint32_t d_tmem;
-  uint64_t adesc, bdesc;
-  uint32_t idesc, accumulate;
-};
-
 struct Cluster;
 struct Cta {
   std::vector<unsigned char> smem_store;
   unsigned char* smem = nullptr;  // 1024-aligned arena
   size_t smem_bytes = 0;
-  std::vector<float> tmem;  // [128][512]
   Barrier sync_all;
-  Barrier named[16];
   Barrier warp_bar[64];
   double warp_scratch[64][32];
-  std::map<uint32_t, MBar> mbars;
   dim3 block_idx;
   unsigned rank = 0;
   Cluster* cluster = nullptr;
@@ -124,13 +92,10 @@ struct Cta {
 struct Cluster {
   std::vector<Cta> ctas;
   Barrier sync;  // barrier.cluster
-  std::mutex mb_m;  // guards every mbarrier of the cluster + TMEM / MMA execution
-  std::condition_variable mb_cv;
 };
 
 inline thread_local dim3 t_threadIdx, t_blockIdx;
 inline thread_local Cta* t_cta = nullptr;
-inline thread_local std::vector<MmaRec>* t_mma_queue = nullptr;
 inline dim3 g_blockDim, g_gridDim;
 
 inline unsigned linear_tid() {
@@ -226,7 +191,7 @@ template <typename F>
 inline cudaError_t cudaFuncSetAttribute(F, cudaFuncAttribute, int) { return cudaSuccess; }
 inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
 struct cudaDeviceProp { int multiProcessorCount; int major; int minor; };
-inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) { p->multiProcessorCount = 4; p->major = 10; p->minor = 0; return cudaSuccess; }
+inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) { p->multiProcessorCount = 4; p->major = 9; p->minor = 0; return cudaSuccess; }
 
 typedef void* cudaEvent_t;
 inline cudaError_t cudaEventCreate(cudaEvent_t* e) { *e = nullptr; return cudaSuccess; }
@@ -237,8 +202,7 @@ inline cudaError_t cudaEventElapsedTime(float* t, cudaEvent_t, cudaEvent_t) { *t
 
 namespace emul {
 // Run `body` once per (block, thread).  Clusters (groups of `cluster_x` consecutive blocks along x) run one after
-// the other; the threads of a cluster's CTAs are real OS threads, so __syncthreads / mbarrier / cluster-barrier
-// semantics are honest.
+// the other; the threads of a cluster's CTAs are real OS threads, so __syncthreads semantics are honest.
 inline void launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()>& body, unsigned cluster_x = 1) {
   g_blockDim = block;
   g_gridDim = grid;
@@ -266,13 +230,10 @@ inline void launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function
         for (unsigned r = 0; r < cluster_x; ++r)
           for (unsigned t = 0; t < nthr; ++t) {
             th.emplace_back([=, &body, &cl]() {
-              std::vector<MmaRec> q;
-              t_mma_queue = &q;
               t_cta = &cl.ctas[r];
               t_blockIdx = cl.ctas[r].block_idx;
               t_threadIdx = dim3(t % block.x, (t / block.x) % block.y, t / (block.x * block.y));
               body();
-              if (!q.empty()) die("thread exited with tcgen05.mma instructions that were never committed");
             });
           }
         for (auto& x : th) x.join();
@@ -296,209 +257,3 @@ inline float4 make_float4(float x, float y, float z, float w) { return float4{x,
 inline float2 make_float2(float x, float y) { return float2{x, y}; }
 inline uint4 make_uint4(uint32_t x, uint32_t y, uint32_t z, uint32_t w) { return uint4{x, y, z, w}; }
 inline uint2 make_uint2(uint32_t x, uint32_t y) { return uint2{x, y}; }
-
-// =====================================================================================================
-// tcgen05 / mbarrier / TMEM / bulk-copy / cluster emulation
-// =====================================================================================================
-namespace emul {
-
-inline uint32_t smem_addr_of(const void* p) {
-  const unsigned char* c = reinterpret_cast<const unsigned char*>(p);
-  if (c < t_cta->smem || c >= t_cta->smem + t_cta->smem_bytes + 1024) die("smem_u32 of a pointer outside the CTA's shared arena");
-  return (uint32_t)(c - t_cta->smem) + SMEM_BASE;
-}
-inline unsigned char* smem_ptr(Cta* c, uint32_t addr) {
-  if (addr < SMEM_BASE || addr - SMEM_BASE >= c->smem_bytes + 1024) die("shared-window address out of range");
-  return c->smem + (addr - SMEM_BASE);
-}
-
-// ---- mbarrier ----
-inline MBar& mbar_ref(Cta* c, uint32_t addr, bool must_exist = true) {
-  MBar& b = c->mbars[addr];
-  if (must_exist && !b.valid) die("mbarrier used before mbarrier.init");
-  return b;
-}
-inline void mbar_complete_if_ready(Cluster* cl, MBar& b) {
-  if (b.pending == 0 && b.tx == 0) {
-    b.phase ^= 1u;
-    b.pending = b.init_count;
-    cl->mb_cv.notify_all();
-  }
-}
-inline void mbar_init(uint32_t addr, uint32_t count) {
-  Cluster* cl = t_cta->cluster;
-  std::lock_guard<std::mutex> lk(cl->mb_m);
-  MBar& b = t_cta->mbars[addr];
-  b.init_count = b.pending = count;
-  b.tx = 0;
-  b.phase = 0;
-  b.valid = true;
-}
-inline void mbar_arrive_on(Cta* c, uint32_t addr, long long expect_tx) {
-  Cluster* cl = c->cluster;
-  std::lock_guard<std::mutex> lk(cl->mb_m);
-  MBar& b = mbar_ref(c, addr);
-  if (b.pending == 0) die("mbarrier arrival count underflow (more arrivals than the barrier was initialised for)");
-  b.tx += expect_tx;
-  --b.pending;
-  mbar_complete_if_ready(cl, b);
-}
-inline void mbar_complete_tx(Cta* c, uint32_t addr, long long bytes) {
-  Cluster* cl = c->cluster;
-  std::lock_guard<std::mutex> lk(cl->mb_m);
-  MBar& b = mbar_ref(c, addr);
-  b.tx -= bytes;
-  mbar_complete_if_ready(cl, b);
-}
-inline bool mbar_test(uint32_t addr, uint32_t parity) {
-  Cluster* cl = t_cta->cluster;
-  std::lock_guard<std::mutex> lk(cl->mb_m);
-  return mbar_ref(t_cta, addr).phase != (parity & 1u);
-}
-inline void mbar_wait_block(uint32_t addr, uint32_t parity) {
-  Cluster* cl = t_cta->cluster;
-  std::unique_lock<std::mutex> lk(cl->mb_m);
-  MBar& b = mbar_ref(t_cta, addr);
-  const bool ok = cl->mb_cv.wait_for(lk, std::chrono::seconds(90), [&] { return b.phase != (parity & 1u); });
-  if (!ok) {
-    fprintf(stderr, "[cuda_emul] mbarrier wait timed out: cta rank %u addr %u parity %u (phase %u pending %u tx %lld)\n",
-            t_cta->rank, addr, parity, b.phase, b.pending, b.tx);
-    die("deadlock on an mbarrier");
-  }
-}
-
-// ---- TMEM ----
-inline float& tmem_at(Cta* c, uint32_t lane, uint32_t col) {
-  if (lane >= 128 || col >= 512) die("TMEM access out of range");
-  return c->tmem[(size_t)lane * 512 + col];
-}
-inline void tmem_alloc(uint32_t dst_smem_addr, uint32_t ncols) {
-  if (ncols < 32 || ncols > 512 || (ncols & (ncols - 1))) die("tcgen05.alloc: column count must be a power of two in [32, 512]");
-  if ((linear_tid() & 31) == 0) {
-    if (t_cta->tmem.empty()) t_cta->tmem.assign((size_t)128 * 512, NAN);
-    const uint32_t base = 0;
-    memcpy(smem_ptr(t_cta, dst_smem_addr), &base, 4);
-  }
-}
-// tcgen05.ld.32x32b.x32: thread i of the warp reads lane (quadrant base + i), 32 consecutive columns
-inline void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  const uint32_t lane0 = taddr >> 16, col0 = taddr & 0xFFFFu;
-  const unsigned t = linear_tid();
-  if (lane0 != 32u * ((t >> 5) & 3u)) die("tcgen05.ld: a warp may only access the TMEM lanes of its own quadrant (warp % 4)");
-  Cluster* cl = t_cta->cluster;
-  std::lock_guard<std::mutex> lk(cl->mb_m);
-  for (int j = 0; j < 32; ++j) {
-    const float v = tmem_at(t_cta, lane0 + (t & 31), col0 + j);
-    memcpy(&r[j], &v, 4);
-  }
-}
-
-// ---- UMMA ----
-inline uint32_t desc_start(uint64_t d) { return (uint32_t)(d & 0x3FFFu) << 4; }
-inline uint32_t desc_sbo(uint64_t d) { return (uint32_t)((d >> 32) & 0x3FFFu) << 4; }
-// element address of (row, byte offset kb within the instruction's K extent) for K-major SWIZZLE_128B
-inline uint32_t umma_addr(uint64_t desc, int row, int kb) {
-  if (((desc >> 61) & 7u) != 2u) die("tcgen05.mma emulation only knows SWIZZLE_128B K-major operands");
-  const uint32_t lin = desc_start(desc) + (uint32_t)(row >> 3) * desc_sbo(desc) + (uint32_t)(row & 7) * 128u + (uint32_t)kb;
-  return lin ^ (((lin >> 7) & 7u) << 4);
-}
-inline float half_to_float(uint16_t h) {
-  const uint32_t s = (h >> 15) & 1u, e = (h >> 10) & 31u, m = h & 1023u;
-  float v;
-  if (e == 0) v = ldexpf((float)m, -24);
-  else if (e == 31) v = m ? NAN : INFINITY;
-  else v = ldexpf((float)(m | 1024u), (int)e - 25);
-  return s ? -v : v;
-}
-inline float bf16_to_float(uint16_t h) { uint32_t u = (uint32_t)h << 16; float f; memcpy(&f, &u, 4); return f; }
-inline float acc_round(double x) {
-  static const bool rn = getenv("PPSCI_EMUL_ACC_RN") != nullptr;
-  float f = (float)x;  // round to nearest
-  if (rn || std::isnan(f) || std::isinf(f)) return f;
-  if (fabs((double)f) > fabs(x)) f = nextafterf(f, 0.0f);  // toward zero
-  return f;
-}
-inline void exec_mma(Cluster* cl, Cta* leader, const MmaRec& m) {
-  const int M = (int)((m.idesc >> 24) & 31u) << 4, N = (int)((m.idesc >> 17) & 63u) << 3;
-  const int ncta = m.group;
-  if (ncta == 2 && M != 256) die("cta_group::2 emulation expects M = 256");
-  if (ncta == 1 && M != 128) die("cta_group::1 emulation expects M = 128");
-  if (N < 16 || N > 256 || (N % 16)) die("tcgen05.mma: bad N");
-  const int kelems = m.kind == 0 ? 8 : 16, es = m.kind == 0 ? 4 : 2;
-  auto ld = [&](Cta* c, uint64_t desc, int row, int k) -> double {
-    const unsigned char* p = smem_ptr(c, umma_addr(desc, row, k * es));
-    if (m.kind == 0) {
-      uint32_t u;
-      memcpy(&u, p, 4);
-      u &= 0xFFFFE000u;  // tf32: 10 explicit mantissa bits, the rest is ignored
-      float f;
-      memcpy(&f, &u, 4);
-      return (double)f;
-    }
-    uint16_t h;
-    memcpy(&h, p, 2);
-    return (double)(m.kind == 1 ? half_to_float(h) : bf16_to_float(h));
-  };
-  const int nper = N / ncta;  // B rows supplied by each CTA
-  std::vector<double> B((size_t)N * kelems);
-  for (int n = 0; n < N; ++n) {
-    Cta* src = ncta == 2 ? &cl->ctas[n / nper] : leader;
-    for (int k = 0; k < kelems; ++k) B[(size_t)n * kelems + k] = ld(src, m.bdesc, n % nper, k);
-  }
-  const uint32_t dcol = m.d_tmem & 0xFFFFu;
-  if ((m.d_tmem >> 16) != 0) die("tcgen05.mma: accumulator address must start at lane 0");
-  for (int r = 0; r < M; ++r) {
-    Cta* c = ncta == 2 ? &cl->ctas[r / 128] : leader;
-    double a[16];
-    for (int k = 0; k < kelems; ++k) a[k] = ld(c, m.adesc, r % 128, k);
-    for (int n = 0; n < N; ++n) {
-      double s = 0;
-      for (int k = 0; k < kelems; ++k) s += a[k] * B[(size_t)n * kelems + k];
-      float& d = tmem_at(c, (uint32_t)(r % 128), dcol + (uint32_t)n);
-      d = m.accumulate ? acc_round((double)d + s) : acc_round(s);
-    }
-  }
-}
-inline void mma_issue(int group, int kind, uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if (group == 2 && t_cta->rank != 0) die("cta_group::2 MMAs are issued by the leader CTA (rank 0)");
-  t_mma_queue->push_back(MmaRec{group, kind, d_tmem, adesc, bdesc, idesc, accumulate});
-}
-// tcgen05.commit: everything this thread issued so far has executed -> arrive on the barrier (multicast for pairs)
-inline void mma_commit(int group, uint32_t bar_addr, unsigned cta_mask) {
-  Cluster* cl = t_cta->cluster;
-  {
-    std::lock_guard<std::mutex> lk(cl->mb_m);
-    for (const MmaRec& m : *t_mma_queue) exec_mma(cl, t_cta, m);
-    t_mma_queue->clear();
-  }
-  if (group == 1) {
-    mbar_arrive_on(t_cta, bar_addr, 0);
-  } else {
-    for (unsigned r = 0; r < cl->ctas.size(); ++r)
-      if (cta_mask & (1u << r)) mbar_arrive_on(&cl->ctas[r], bar_addr, 0);
-  }
-}
-
-// ---- copies ----
-inline void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
-  if (bytes % 16 || (dst_smem % 16) || (reinterpret_cast<uintptr_t>(src) % 16)) die("cp.async.bulk: size / addresses must be 16-byte aligned");
-  memcpy(smem_ptr(t_cta, dst_smem), src, bytes);
-  mbar_complete_tx(t_cta, bar, bytes);
-}
-inline void cp_async16(uint32_t dst_smem, const void* src, bool valid) {
-  if (valid) memcpy(smem_ptr(t_cta, dst_smem), src, 16);
-  else memset(smem_ptr(t_cta, dst_smem), 0, 16);
-}
-
-inline float tf32_rna(float x) {
-  uint32_t u;
-  memcpy(&u, &x, 4);
-  if (((u >> 23) & 0xFFu) == 0xFFu) return x;
-  u += 0x1000u;
-  u &= 0xFFFFE000u;
-  float r;
-  memcpy(&r, &u, 4);
-  return r;
-}
-
-}  // namespace emul

@@ -33,24 +33,3 @@ def test_tile_gemm_path_for_thin_layers(emul_lib, name, monkeypatch):
     tl, tr, tg = TOL[CASES[name]["dtype"]]
     assert r["loss"] <= tl and r["res"] <= tr and r["grad"] <= tg, r
 
-
-# PPSCI_B200_TC_MASK: 255 = default (fp16-operand fused forward for 256-wide layers + fused dx chain + pair dW),
-# 511 = tf32 fused forward (+ fused dx), 63 = layer-at-a-time CTA-pair kernels only
-@pytest.mark.parametrize("mask", [255, 511, 63])
-def test_tcgen05_kernels_through_the_emulated_primitives(emul_lib, mask, monkeypatch):
-    """The tensor-core kernels (layer-fused k_fused_fwd16 / k_fused_fwd / k_fused_dx, CTA-pair k_tc2_fwd / k_tc2_dx /
-    k_tc2_dw, thin first / last layers) compiled for the CPU: UMMA descriptors decoded, 128-byte swizzle, mbarrier
-    phases, TMEM lane quadrants, cta_group::2 operand split, kind::tf32 / kind::f16 operands, round-toward-zero
-    accumulation, MMAs executed at the commit (tests/emul/cuda_emul.h).  60 points = 3 point tiles: one full tile pair
-    + a pair whose second CTA has an empty tile; 3 x 256 hidden layers = two fused layers."""
-    monkeypatch.setenv("PPSCI_B200_TC_MASK", str(mask))
-    case = dict(in_keys=("x", "y"), out_keys=("u", "v", "p"), hidden=[256] * 3, act="tanh",
-                exprs=lambda: __import__("oracle.ppsci_oracle", fromlist=["x"]).navier_stokes_expr(0.01, 1.0, 2, False),
-                dtype=torch.float32)
-    r = run_case(case, 60, library=emul_lib, device="cpu", backend=2)
-    assert r["tc"]
-    # the tf32 fused forward keeps ONE accumulator per 256-wide layer: not the default there because of exactly this
-    # (DESIGN.md section 4.1); it is exercised here as the cross-check of the shared ring / barrier protocol
-    tol = 3e-5 if mask == 511 else 1e-5
-    assert r["loss"] <= tol and r["res"] <= tol and r["grad"] <= 2e-5, r
-    assert r["fwd_vs_fused"] == 0.0, r

@@ -9,7 +9,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_case_matches_oracle_gpu(name):
-    assert torch.cuda.is_available(), "GPU tests need a B200"
+    assert torch.cuda.is_available(), "GPU tests need an H100"
     n = 3000 if CASES[name]["hidden"][0] > 64 else 5000
     r = run_case(name, n, device="cuda:0", backend=1)
     tl, tr, tg = TOL[CASES[name]["dtype"]]

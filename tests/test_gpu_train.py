@@ -1,4 +1,4 @@
-"""End-to-end training steps through the public API on a B200 (Solver.train: fused loss + weight-gradient call per
+"""End-to-end training steps through the public API on an H100 (Solver.train: fused loss + weight-gradient call per
 constraint -> optimizer) against the same optimizer driven by the oracle's loss / gradient in fp64.
 
 Reference loops: ppsci/solver/train.py:58-213 (Adam), :216-319 (L-BFGS closure)."""

@@ -133,24 +133,6 @@ def test_subnet_weight_norm_and_skip_connection_through_emulated_kernels(monkeyp
     assert list(sd2) == list(sd) and all(torch.equal(sd2[k], sd[k]) for k in sd)
 
 
-def test_wide_output_layer_on_the_emulated_tensor_core_kernels(monkeypatch):
-    """The sub-networks end in ``num_features`` (128) units: that output layer and its dW run on the tensor-core kernels
-    (fp32, forced here with backend 2 because the emulated tcgen05 path runs on request only), like the hidden layers."""
-    from tests.emul.build_emul import build
-
-    monkeypatch.setattr(B, "_default", B.Library(build()))
-    monkeypatch.setenv("PPSCI_B200_BACKEND", "2")
-    hidden = [128, 128]
-    model, cst, data = _setup(torch.float32, "cpu", 150, 100, 128, hidden)  # num_loc = 100: the dense first layer takes the tensor-core path too (K padded to 128)
-    losses_all, _ = _train_forward(model, cst, "cpu", torch.float32)
-    plans = model._get_plans()
-    assert all(p.uses_tcgen05 for p in plans)
-    _, loss, grad = _oracle(model, cst, hidden)
-    assert abs(float(losses_all["G"]) - loss) <= 2e-5 * abs(loss)
-    got = model.flat.grad.detach().double()
-    assert float((got - grad).norm() / grad.norm()) <= 5e-5
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("options", [{}, dict(branch_weight_norm=True, trunk_skip_connection=True)])
 def test_cfg5_shapes_on_gpu_match_oracle(options):
