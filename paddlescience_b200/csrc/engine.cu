@@ -1014,7 +1014,7 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         break;
       }
 #ifndef PPSCI_EMUL
-      if (sizeof(T) == 4 && wg_dw_layer(P, l)) {  // dW_l on the tensor cores, db_l beside it
+      if (sizeof(T) == 4 && wg_dw_layer(P, l)) {  // dW_l and db_l on the tensor cores
         wg::WgDwArgs w;
         memset(&w, 0, sizeof(w));
         if (l == 1) {  // dense first layer: the caller's matrix is the operand
@@ -1028,32 +1028,27 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         w.ldzb = zbar_ld;
         w.zbplane = (long long)nc_max * zbar_ld;
         w.Kdim = s.widths[l - 1];
+        w.Nout = s.widths[l];
         w.dW = reinterpret_cast<float*>(grads) + P->w_off[l];
+        w.db = reinterpret_cast<float*>(grads) + P->b_off[l];
         w.Np = nc;
-        const int N = s.widths[l], PTw = wg::KCH / C;
-        const long long total_chunks = (nc + PTw - 1) / PTw;
-        const unsigned kt = (unsigned)((w.Kdim + wg::TM - 1) / wg::TM);
-        long long want = P->num_sms / kt;
+        // column blocks of equal width (in units of 32) up to dw_maxq(C); fan-in blocks x column blocks fastest on the
+        // grid, so the CTAs that read the same points run together and share them through L2
+        const int nq = w.Nout / 32, ncb = (nq + wg::dw_maxq(C) - 1) / wg::dw_maxq(C), bnq = (nq + ncb - 1) / ncb;
+        w.col_blocks = ncb;
+        const long long total_chunks = (nc + wg::dw_pch(C) - 1) / wg::dw_pch(C);
+        const unsigned tiles = (unsigned)((w.Kdim + wg::DW_TK - 1) / wg::DW_TK * ncb);
+        long long want = P->num_sms / tiles;
         if (want < 1) want = 1;
         if (want > total_chunks) want = total_chunks;
         const long long cps = (total_chunks + want - 1) / want;
         w.chunks_per_split = (int)cps;
         const unsigned splits = (unsigned)((total_chunks + cps - 1) / cps);
-        const int smem = wg::fwd_smem_bytes(N);
-        {
-          ProfScope ps_(P, CLS_DW, st);
-          PPSCI_WG_DW_LAUNCH(wg_layout(P->J), N, dim3(kt, splits), smem, st, w,
-                             return fail(std::string("cudaFuncSetAttribute(k_wg_dw): ") + cudaGetErrorString(e_)));
-          P->launches++;
-        }
-        {
-          ProfScope ps_(P, CLS_THIN_DW, st);
-          const int ppb = 512;
-          PPSCI_LAUNCH(wg::k_wg_bias_grad, dim3((unsigned)((N + 127) / 128), (unsigned)((nc + ppb - 1) / ppb)), dim3(128), 0, st,
-                       reinterpret_cast<const float*>(zbar_cur), zbar_ld, (long long)nc, N,
-                       reinterpret_cast<float*>(grads) + P->b_off[l], ppb);
-          P->launches++;
-        }
+        const int smem = wg::dw_smem_bytes(C, bnq);
+        ProfScope ps_(P, CLS_DW, st);
+        PPSCI_WG_DW_LAUNCH(wg_layout(P->J), bnq, dim3(tiles, splits), smem, st, w,
+                           return fail(std::string("cudaFuncSetAttribute(k_wg_dw): ") + cudaGetErrorString(e_)));
+        P->launches++;
       } else
 #endif
       {  // dW_l, db_l

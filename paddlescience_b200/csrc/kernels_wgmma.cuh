@@ -409,177 +409,273 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_layer(WgArgs g) {
   }
 }
 
-// ---- weight gradient  dW_l[k][n] += sum over jet rows  a_{l-1}[row][k] Zbar_l[row][n] ------------------------------
-// The contraction runs over jet rows, so both operands are transposes of the row-major jet planes: the A tile holds 64
-// fan-in rows k x 32 jet rows (PT = 32 / C points x C channels per chunk, the activation jets of Z_{l-1} recomputed on
-// the fly), the B tile N output columns x the same 32 jet rows (Zbar_l); both split hi / lo into the same K-major
-// 128-byte-swizzled stages as k_wg_layer, and the same two warpgroups accumulate A_hi B_hi and the cross terms.  CTA
-// (kb, split) owns dW rows [64 kb, +64) and a contiguous range of chunks; it flushes once with atomicAdd.
+// ---- weight gradient  dW_l[k][n] += sum over jet rows  a_{l-1}[row][k] Zbar_l[row][n],  db_l[n] += sum_p Zbar_l[0][p][n] ----
+// The contraction runs over jet rows, in any order both operands share.  K index 4 j + u is point 4 q + u of channel c,
+// j = c + C q (point quads, channels within a quad), so every aligned group of 4 K elements is 4 consecutive points of
+// one channel and no jet row is left unused, for any C.  A chunk is dw_pch(C) points = dw_groups(C) groups, issued as dw_ksteps(C) K steps
+// of 8 (an odd group count is padded with one zero group).
+//
+// A = act_jets(Z_{l-1})^T comes from registers: the tf32 A fragment gives lane t = lane % 4 of warp w the K elements
+// 8 s + t and 8 s + t + 4 of rows 16 w + lane / 4 (+ 8), i.e. only points = t (mod 4).  Each thread computes the jets of
+// its own (point, fan-in row) pairs once per CTA and splits them hi / lo in registers.
+// B = Zbar_l^T is staged per chunk, K-major with the 128-byte swizzle: thread <-> output column, 32 lanes read 128
+// contiguous bytes of one row, and each (column, group) is one float4 of hi and one of lo at sw128_q(column, group), so
+// eight consecutive columns land in eight distinct 16-byte bank groups.
+//
+// CTA (fan-in block of 128 rows, column block of BN <= 128 columns, range of chunks): warpgroup i owns fan-in rows
+// 64 i .. 64 i + 63 and issues  A_hi B_hi -> exact accumulator,  A_lo B_hi + A_hi B_lo -> cross accumulator  per K step
+// (the 3xTF32 scheme of k_wg_layer, with the exact-product term in an accumulator of its own).  While the MMAs of chunk j
+// run, the Zbar_l values of chunk j + 1 are loaded into registers and written to the other B stage, and its Z_{l-1}
+// values are copied into per-thread shared-memory slots by cp.async (they would not fit in registers beside the two
+// accumulators and the in-flight A fragments); the jets are computed once those MMAs have retired.  The CTA flushes once
+// with atomicAdd; the CTAs of fan-in block 0 also add their columns' channel-0 sums (summed in shared memory) to db_l.
+__host__ __device__ constexpr int dw_pch(int C) { return C >= 8 ? 4 : C >= 3 ? 8 : 32 / C; }  // points per chunk
+__host__ __device__ constexpr int dw_groups(int C) { return dw_pch(C) / 4 * C; }
+__host__ __device__ constexpr int dw_ksteps(int C) { return (dw_groups(C) + 1) / 2; }
+__host__ __device__ constexpr int dw_atoms(int C) { return (dw_ksteps(C) + 3) / 4; }  // 32-wide K atoms per B stage
+// widest column block in units of 32: two accumulators of BN / 2 registers each, beside the A fragments and the B
+// prefetch of a chunk, must fit in 255 registers without spilling
+__host__ __device__ constexpr int dw_maxq(int C) { return C <= 5 ? 4 : C <= 8 ? 2 : 1; }
+__host__ __device__ constexpr int dw_q(int C, int q) { return q < dw_maxq(C) ? q : dw_maxq(C); }
+// two stages of [hi | lo][atoms][BN rows x 128 bytes], 1024-byte aligned, then the db_l column sums and the A operand's
+// per-thread Z_{l-1} slots
+__host__ __device__ constexpr int dw_smem_bytes(int C, int bnq) {
+  return 2 * 2 * dw_atoms(C) * bnq * 32 * 128 + bnq * 32 * 4 + dw_pch(C) / 4 * 2 * C * 256 * 4 + 1024;
+}
+constexpr int DW_TK = 128;  // fan-in rows per CTA
+
 struct WgDwArgs {
   AOperand<float> A;   // A_ACT over Z_{l-1}
   JetLayout J;
   const float* Zbar;   // [C][Np][ldzb]
   int ldzb;
   long long zbplane;
-  int Kdim;            // fan-in (rows of dW), a multiple of 4
-  float* dW;           // [Kdim][N]
+  int Kdim;            // fan-in (rows of dW)
+  int Nout;            // fan-out (columns of dW)
+  int col_blocks;      // column blocks per fan-in block (blockIdx.x = fan-in block * col_blocks + column block)
+  float* dW;           // [Kdim][Nout]
+  float* db;           // [Nout]
   long long Np;
   int chunks_per_split;
 };
 
-template <class L, int NQ>
+// D[64 x 64] += A[64 x 8] B[8 x 64], A tf32 fragments in registers, B from shared memory
+__device__ __forceinline__ void wgmma_tf32_rA_m64n64(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1u));
+}
+// D[64 x 32] += A[64 x 8] B[8 x 32]
+__device__ __forceinline__ void wgmma_tf32_rA_m64n32(float (&d)[16], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1u));
+}
+
+// activation jets y[0 .. CS) of one (point, unit) from its pre-activation jets z[0 .. CS)
+template <class L>
+__device__ __forceinline__ void act_jets(int act, const JetLayout& J, const float (&z)[L::CS], float (&y)[L::CS]) {
+  float sc[6];
+  act_coef<float, L::KM>(act, z[0], y[0], sc);
+#pragma unroll
+  for (int d = 0; d < L::ND; ++d) {
+    const int K = L::order(J, d), cb = L::cbase(J, d);
+    float zz[4], yy[4];
+#pragma unroll
+    for (int o = 0; o < 4; ++o) zz[o] = (o < L::KM && o < K) ? z[(cb + o) < L::CS ? (cb + o) : 0] : 0.f;
+    jet_fwd_dir<float, L::KM>(sc, zz, yy);
+#pragma unroll
+    for (int o = 0; o < L::KM; ++o)
+      if (o < K && cb + o < L::CS) y[cb + o] = yy[o];
+  }
+}
+
+template <class L, int BNQ>
 __global__ void __launch_bounds__(THREADS, 1) k_wg_dw(WgDwArgs g) {
   PPSCI_DYN_SMEM(smem_dyn);
   const uint32_t base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
   unsigned char* base_ptr = smem_dyn + (base - smem_u32(smem_dyn));
-  constexpr int CS = L::CS;
-  constexpr int PT = KCH / CS;  // points per chunk of 32 jet rows
-  constexpr int N = NQ * 32;
-  constexpr int NB = NQ / 2, TAIL = NQ & 1;
-  const int sbytes = stage_bytes(N);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wgi = tid >> 7;
-  const int k0 = blockIdx.x * TM;
-  const long long total_chunks = (g.Np + PT - 1) / PT;
-  const long long ch_begin = (long long)blockIdx.y * g.chunks_per_split;
-  const long long ch_end = ch_begin + g.chunks_per_split < total_chunks ? ch_begin + g.chunks_per_split : total_chunks;
+  constexpr int CS = L::CS, PCH = dw_pch(CS), QPC = PCH / 4, G = dw_groups(CS), KS = dw_ksteps(CS), NA = dw_atoms(CS);
+  constexpr int BN = BNQ * 32, NB = BNQ / 2, TAIL = BNQ & 1;
+  constexpr int ATOM = BN * 128;                            // bytes of one K atom of B (hi or lo)
+  constexpr int STAGE = 2 * NA * ATOM;
+  constexpr int BI = (G * BN + THREADS - 1) / THREADS;     // B items (group, column) per thread and chunk
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wgi = tid >> 7, t = lane & 3;
+  const int kb = blockIdx.x / g.col_blocks, n0 = (blockIdx.x - kb * g.col_blocks) * BN;
+  const int Np = (int)g.Np;  // points per call < 2^31 (the workspace chunk)
+  const int total_chunks = (Np + PCH - 1) / PCH;
+  const int ch_begin = blockIdx.y * g.chunks_per_split;
+  const int ch_end = ch_begin + g.chunks_per_split < total_chunks ? ch_begin + g.chunks_per_split : total_chunks;
+  if (ch_begin >= ch_end) return;
   const int act = g.A.act;
+  const int krow = kb * DW_TK + wgi * 64 + (warp & 3) * 16 + (lane >> 2);  // A fragment rows krow, krow + 8
 
-  for (int i = tid; i < (2 * sbytes + A_TILE_BYTES) / 16; i += THREADS)  // pad jet rows (>= C PT), the zero tile
+  float* bsum = reinterpret_cast<float*>(base_ptr + 2 * STAGE);  // [BN] channel-0 column sums (fan-in block 0)
+  for (int i = tid; i < (2 * STAGE + BN * 4) / 16; i += THREADS)  // the pad group and the K atoms past the last group stay zero
     reinterpret_cast<float4*>(base_ptr)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  fence_proxy_async();
-  __syncthreads();
+  __syncthreads();  // ... before the first chunk's B writes
 
-  float acc[NB > 0 ? NB : 1][32], acct[TAIL ? 16 : 1];
-  auto frag = [&](int j, int i) -> float& { return j < 8 * NB ? acc[j >> 3][4 * (j & 7) + i] : acct[4 * (j - 8 * NB) + i]; };
+  float ex[NB > 0 ? NB : 1][32], ext[TAIL ? 16 : 1], cr[NB > 0 ? NB : 1][32], crt[TAIL ? 16 : 1];
 #pragma unroll
-  for (int j = 0; j < N / 8; ++j)
+  for (int nb = 0; nb < NB; ++nb)
 #pragma unroll
-    for (int i = 0; i < 4; ++i) frag(j, i) = 0.f;
-  auto put = [&](unsigned char* tile_hi, int tile_lo_off, int row, int col, float v) {
-    const float h = tf32_rn(v);
-    *reinterpret_cast<float*>(tile_hi + sw128(row, col)) = h;
-    *reinterpret_cast<float*>(tile_hi + tile_lo_off + sw128(row, col)) = v - h;
+    for (int i = 0; i < 32; ++i) ex[nb][i] = cr[nb][i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < (TAIL ? 16 : 1); ++i) ext[i] = crt[i] = 0.f;
+
+  // Z_{l-1} at point 4 qq + t of the chunk, fan-in row krow + 8 h, channel c: thread-private slots, filled by cp.async
+  // (zero past Np and Kdim) while the previous chunk's MMAs run
+  float* za = reinterpret_cast<float*>(base_ptr + 2 * STAGE + BN * 4);
+  auto za_at = [&](int qq, int h, int c) -> float* { return za + ((qq * 2 + h) * CS + c) * THREADS + tid; };
+  float4 zb[BI];         // Zbar_l at the 4 points of group gi, column n0 + n, for item tid + THREADS i = gi BN + n
+  auto load_a = [&](int ch) {
+    const int p0 = ch * PCH;
+#pragma unroll
+    for (int qq = 0; qq < QPC; ++qq)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int p = p0 + 4 * qq + t;
+        const int k = krow + 8 * h;
+        const bool ok = p < Np && k < g.Kdim;
+        const float* src = g.A.Z + (ok ? (long long)p * g.A.ld + k : 0);
+#pragma unroll
+        for (int c = 0; c < CS; ++c)
+          asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(za_at(qq, h, c))),
+                       "l"(src + (ok ? (long long)c * g.A.plane : 0)), "r"(ok ? 4 : 0)
+                       : "memory");
+      }
+    asm volatile("cp.async.commit_group;" ::: "memory");
   };
-  uint32_t it = 0;
-  for (long long ch = ch_begin; ch < ch_end; ++ch, ++it) {
-    const uint32_t s = it & 1u;
-    wgmma_wait<1>();
-    __syncthreads();
-    const uint32_t st_addr = base + s * sbytes;
-    unsigned char* st_ptr = base_ptr + s * sbytes;
-    const long long p0 = ch * PT;
-    // A: item = (point, 4 consecutive fan-in rows)
-    for (int item = tid; item < PT * (TM / 4); item += THREADS) {
-      const int pl = item / (TM / 4), kq = item - pl * (TM / 4);
-      const long long p = p0 + pl;
-      const bool valid = p < g.Np && k0 + 4 * kq < g.Kdim;
-      const float* src = g.A.Z + p * g.A.ld + k0 + 4 * kq;
-      float4 z[CS];
+  auto load_b = [&](int ch) {
+    const int p0 = ch * PCH;
 #pragma unroll
-      for (int c = 0; c < CS; ++c)
-        z[c] = valid ? __ldg(reinterpret_cast<const float4*>(src + (long long)c * g.A.plane)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      float yout[CS][4];
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        auto comp = [&](const float4& v) { return t == 0 ? v.x : t == 1 ? v.y : t == 2 ? v.z : v.w; };
-        float sc[6];
-        float y0;
-        act_coef<float, L::KM>(act, comp(z[0]), y0, sc);
-        yout[0][t] = valid ? y0 : 0.f;
-#pragma unroll
-        for (int d = 0; d < L::ND; ++d) {
-          const int K = L::order(g.J, d), cb = L::cbase(g.J, d);
-          float zz[4], yy[4];
-#pragma unroll
-          for (int o = 0; o < 4; ++o) zz[o] = (o < L::KM && o < K) ? comp(z[(cb + o) < CS ? (cb + o) : 0]) : 0.f;
-          jet_fwd_dir<float, L::KM>(sc, zz, yy);
-#pragma unroll
-          for (int o = 0; o < L::KM; ++o)
-            if (o < K && cb + o < CS) yout[cb + o][t] = valid ? yy[o] : 0.f;
-        }
-      }
-#pragma unroll
-      for (int c = 0; c < CS; ++c)
-#pragma unroll
-        for (int t = 0; t < 4; ++t) put(st_ptr, A_TILE_BYTES, 4 * kq + t, c * PT + pl, yout[c][t]);
+    for (int i = 0; i < BI; ++i) {
+      const int item = tid + THREADS * i;
+      const int gi = item / BN, n = item - gi * BN;
+      const int qq = gi / CS, c = gi - qq * CS;
+      const int p = p0 + 4 * qq;
+      const bool ok = item < G * BN && n0 + n < g.Nout;
+      const float* src = g.Zbar + (long long)c * g.zbplane + (long long)p * g.ldzb + n0 + n;
+      zb[i].x = ok && p < Np ? __ldg(src) : 0.f;
+      zb[i].y = ok && p + 1 < Np ? __ldg(src + g.ldzb) : 0.f;
+      zb[i].z = ok && p + 2 < Np ? __ldg(src + 2 * g.ldzb) : 0.f;
+      zb[i].w = ok && p + 3 < Np ? __ldg(src + 3 * g.ldzb) : 0.f;
     }
-    // B: item = (point, 4 consecutive output columns)
-    for (int item = tid; item < PT * (N / 4); item += THREADS) {
-      const int pl = item / (N / 4), nq = item - pl * (N / 4);
-      const long long p = p0 + pl;
-      const bool valid = p < g.Np;
+  };
+
+  load_a(ch_begin);
+  load_b(ch_begin);
+  uint32_t ahi[KS][4], alo[KS][4];
+  for (int ch = ch_begin; ch < ch_end; ++ch) {
+    const int sidx = (ch - ch_begin) & 1;
+    const uint32_t st_addr = base + sidx * STAGE;
+    unsigned char* st = base_ptr + sidx * STAGE;
+    // B of this chunk -> stage sidx; its last reader, chunk ch - 2, retired before the previous chunk's barrier
 #pragma unroll
-      for (int c = 0; c < CS; ++c) {
-        const float4 v = valid ? __ldg(reinterpret_cast<const float4*>(g.Zbar + (long long)c * g.zbplane + p * g.ldzb + 4 * nq))
-                               : make_float4(0.f, 0.f, 0.f, 0.f);
-        put(st_ptr + 2 * A_TILE_BYTES, N * 128, 4 * nq, c * PT + pl, v.x);
-        put(st_ptr + 2 * A_TILE_BYTES, N * 128, 4 * nq + 1, c * PT + pl, v.y);
-        put(st_ptr + 2 * A_TILE_BYTES, N * 128, 4 * nq + 2, c * PT + pl, v.z);
-        put(st_ptr + 2 * A_TILE_BYTES, N * 128, 4 * nq + 3, c * PT + pl, v.w);
-      }
+    for (int i = 0; i < BI; ++i) {
+      const int item = tid + THREADS * i;
+      if (item >= G * BN) continue;
+      const int gi = item / BN, n = item - gi * BN;
+      const float4 v = zb[i];
+      float4 hi, lo;
+      hi.x = tf32_rn(v.x); hi.y = tf32_rn(v.y); hi.z = tf32_rn(v.z); hi.w = tf32_rn(v.w);
+      lo.x = v.x - hi.x; lo.y = v.y - hi.y; lo.z = v.z - hi.z; lo.w = v.w - hi.w;
+      const uint32_t off = (gi >> 3) * ATOM + sw128_q(n, gi & 7);
+      *reinterpret_cast<float4*>(st + off) = hi;
+      *reinterpret_cast<float4*>(st + NA * ATOM + off) = lo;
+      if (kb == 0 && gi % CS == 0) atomicAdd(bsum + n, (v.x + v.y) + (v.z + v.w));
     }
+    wgmma_wait<0>();  // the MMAs of chunk ch - 1 have retired: the fragment registers are free
+    // activation jets of this thread's A elements (points past Np give finite jets of 0 against zero B values)
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    float av[QPC][2][CS];
+#pragma unroll
+    for (int qq = 0; qq < QPC; ++qq)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float z[CS];
+#pragma unroll
+        for (int c = 0; c < CS; ++c) z[c] = *za_at(qq, h, c);
+        act_jets<L>(act, g.J, z, av[qq][h]);
+      }
+    if (ch + 1 < ch_end) load_a(ch + 1);
     fence_proxy_async();
-    __syncthreads();
-    const uint64_t a_hi = make_desc(st_addr), a_lo = make_desc(st_addr + A_TILE_BYTES);
-    const uint64_t b_hi = make_desc(st_addr + 2 * A_TILE_BYTES), b_lo = make_desc(st_addr + 2 * A_TILE_BYTES + N * 128);
-    const uint64_t a1 = wgi ? a_lo : a_hi, a2 = wgi ? a_hi : make_desc(base + 2 * sbytes);  // as in k_wg_layer
+    __syncthreads();  // this chunk's B stage is complete
+    // K step s: a0 / a1 = group 2 s (rows krow / krow + 8), a2 / a3 = group 2 s + 1; group gi = channel gi % C of quad
+    // gi / C
+#pragma unroll
+    for (int s = 0; s < KS; ++s)
+#pragma unroll
+      for (int e = 0; e < 2; ++e)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int gi = 2 * s + e;
+          const float v = gi < G ? av[gi / CS][h][gi % CS] : 0.f;
+          const float vh = tf32_rn(v);
+          ahi[s][2 * e + h] = __float_as_uint(vh);
+          alo[s][2 * e + h] = __float_as_uint(v - vh);
+        }
     wgmma_fence();
 #pragma unroll
-    for (int ks = 0; ks < KCH / 8; ++ks) {
-      const uint64_t inc = (uint64_t)(2 * ks);
-      const uint32_t first = (it == 0 && ks == 0) ? 0u : 1u;
+    for (int s = 0; s < KS; ++s) {
+      const uint64_t b_hi = make_desc(st_addr + (s >> 2) * ATOM + (s & 3) * 32);
+      const uint64_t b_lo = b_hi + (uint64_t)(NA * ATOM / 16);
 #pragma unroll
       for (int nb = 0; nb < NB; ++nb) {
-        const uint64_t bo = inc + (uint64_t)(nb * 64 * 128 / 16);
-        wgmma_tf32_m64n64(acc[nb], a1 + inc, b_hi + bo, first);
-        wgmma_tf32_m64n64(acc[nb], a2 + inc, b_lo + bo, 1u);
+        const uint64_t bo = (uint64_t)(nb * 64 * 128 / 16);  // column block nb = B rows 64 nb ..
+        wgmma_tf32_rA_m64n64(ex[nb], ahi[s], b_hi + bo);
+        wgmma_tf32_rA_m64n64(cr[nb], alo[s], b_hi + bo);
+        wgmma_tf32_rA_m64n64(cr[nb], ahi[s], b_lo + bo);
       }
       if constexpr (TAIL) {
-        const uint64_t bo = inc + (uint64_t)(NB * 64 * 128 / 16);
-        wgmma_tf32_m64n32(acct, a1 + inc, b_hi + bo, first);
-        wgmma_tf32_m64n32(acct, a2 + inc, b_lo + bo, 1u);
+        const uint64_t bo = (uint64_t)(NB * 64 * 128 / 16);  // the last 32 columns
+        wgmma_tf32_rA_m64n32(ext, ahi[s], b_hi + bo);
+        wgmma_tf32_rA_m64n32(crt, alo[s], b_hi + bo);
+        wgmma_tf32_rA_m64n32(crt, ahi[s], b_lo + bo);
       }
     }
     wgmma_commit();
+    if (ch + 1 < ch_end) load_b(ch + 1);
   }
   wgmma_wait<0>();
-  __syncthreads();
-  if (it == 0) return;
-  float* xs = reinterpret_cast<float*>(base_ptr + 2 * A_TILE_BYTES);
-  const int lt = tid & 127;
-  if (wgi == 1) {
-#pragma unroll
-    for (int j = 0; j < N / 8; ++j)
-#pragma unroll
-      for (int i = 0; i < 4; ++i) xs[(4 * j + i) * 128 + lt] = frag(j, i);
-  }
-  __syncthreads();
-  if (wgi != 0) return;
-  const int rbase = (warp & 3) * 16 + (lane >> 2);
+
+  // accumulator fragment: element 4 j + 2 h + b of the n8 block j is row krow + 8 h, column 8 j + 2 t + b
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int k = k0 + rbase + 8 * h;
+    const int k = krow + 8 * h;
     if (k >= g.Kdim) continue;
-    float* row = g.dW + (long long)k * N;
+    float* row = g.dW + (long long)k * g.Nout + n0;
 #pragma unroll
-    for (int j = 0; j < N / 8; ++j) {
-      const int col = j * 8 + 2 * (lane & 3);
-      atomicAdd(row + col, frag(j, 2 * h) + xs[(4 * j + 2 * h) * 128 + lt]);
-      atomicAdd(row + col + 1, frag(j, 2 * h + 1) + xs[(4 * j + 2 * h + 1) * 128 + lt]);
+    for (int j = 0; j < BN / 8; ++j) {
+      if (n0 + 8 * j >= g.Nout) break;
+      const int col = 8 * j + 2 * t;
+      const float e0 = j < 8 * NB ? ex[j >> 3][4 * (j & 7) + 2 * h] : ext[4 * (j - 8 * NB) + 2 * h];
+      const float e1 = j < 8 * NB ? ex[j >> 3][4 * (j & 7) + 2 * h + 1] : ext[4 * (j - 8 * NB) + 2 * h + 1];
+      const float c0 = j < 8 * NB ? cr[j >> 3][4 * (j & 7) + 2 * h] : crt[4 * (j - 8 * NB) + 2 * h];
+      const float c1 = j < 8 * NB ? cr[j >> 3][4 * (j & 7) + 2 * h + 1] : crt[4 * (j - 8 * NB) + 2 * h + 1];
+      atomicAdd(row + col, e0 + c0);
+      atomicAdd(row + col + 1, e1 + c1);
     }
   }
-}
-
-// db_l[n] += sum over points of Zbar_l[channel 0][p][n]   (tiny, HBM-bound)
-__global__ void k_wg_bias_grad(const float* __restrict__ Zbar0, int ld, long long Np, int N, float* __restrict__ db,
-                               int pts_per_block) {
-  const int n = blockIdx.x * blockDim.x + threadIdx.x;
-  if (n >= N) return;
-  const long long p_begin = (long long)blockIdx.y * pts_per_block;
-  const long long p_end = p_begin + pts_per_block < Np ? p_begin + pts_per_block : Np;
-  float acc = 0.f;
-  for (long long p = p_begin; p < p_end; ++p) acc += Zbar0[p * ld + n];
-  atomicAdd(db + n, acc);
+  if (kb == 0) {
+    __syncthreads();
+    if (tid < BN && n0 + tid < g.Nout) atomicAdd(g.db + n0 + tid, bsum[tid]);
+  }
 }
 
 }  // namespace wg
@@ -625,24 +721,21 @@ inline bool wg_dw_ok(const ppsci_plan_spec& s, int l, const JetLayout& J) {
   return K % 4 == 0 && N % 32 == 0 && N >= 32 && N <= 256;
 }
 
-#define PPSCI_WG_DW_PICK_(LAY, n)                                                                                \
-  ((n) == 256   ? wg::k_wg_dw<LAY, 8>                                                                           \
-   : (n) == 224 ? wg::k_wg_dw<LAY, 7>                                                                           \
-   : (n) == 192 ? wg::k_wg_dw<LAY, 6>                                                                           \
-   : (n) == 160 ? wg::k_wg_dw<LAY, 5>                                                                           \
-   : (n) == 128 ? wg::k_wg_dw<LAY, 4>                                                                           \
-   : (n) == 96  ? wg::k_wg_dw<LAY, 3>                                                                           \
-   : (n) == 64  ? wg::k_wg_dw<LAY, 2>                                                                           \
-                : wg::k_wg_dw<LAY, 1>)
-#define PPSCI_WG_DW_LAUNCH(lay, n, grid, smem, stream, args, err_expr)                                            \
+// column block of q x 32 columns (q <= dw_maxq(C)); layouts with more channels instantiate only the narrower blocks
+#define PPSCI_WG_DW_PICK_(LAY, q)                                                                                \
+  ((q) == 4   ? wg::k_wg_dw<LAY, wg::dw_q(LAY::CS, 4)>                                                          \
+   : (q) == 3 ? wg::k_wg_dw<LAY, wg::dw_q(LAY::CS, 3)>                                                          \
+   : (q) == 2 ? wg::k_wg_dw<LAY, 2>                                                                             \
+              : wg::k_wg_dw<LAY, 1>)
+#define PPSCI_WG_DW_LAUNCH(lay, q, grid, smem, stream, args, err_expr)                                            \
   do {                                                                                                           \
     void (*kfn_)(decltype(args)) = nullptr;                                                                      \
     switch (lay) {                                                                                               \
-      case LAY_22: kfn_ = PPSCI_WG_DW_PICK_(thin::Lay22, n); break;                                              \
-      case LAY_12: kfn_ = PPSCI_WG_DW_PICK_(thin::Lay12, n); break;                                              \
-      case LAY_222: kfn_ = PPSCI_WG_DW_PICK_(thin::Lay222, n); break;                                            \
-      case WG_LAY_4444: kfn_ = PPSCI_WG_DW_PICK_(wg::Lay4444, n); break;                                         \
-      default: kfn_ = PPSCI_WG_DW_PICK_(thin::LayV, n);                                                          \
+      case LAY_22: kfn_ = PPSCI_WG_DW_PICK_(thin::Lay22, q); break;                                              \
+      case LAY_12: kfn_ = PPSCI_WG_DW_PICK_(thin::Lay12, q); break;                                              \
+      case LAY_222: kfn_ = PPSCI_WG_DW_PICK_(thin::Lay222, q); break;                                            \
+      case WG_LAY_4444: kfn_ = PPSCI_WG_DW_PICK_(wg::Lay4444, q); break;                                         \
+      default: kfn_ = PPSCI_WG_DW_PICK_(thin::LayV, q);                                                          \
     }                                                                                                            \
     cudaError_t e_ = cudaFuncSetAttribute(kfn_, cudaFuncAttributeMaxDynamicSharedMemorySize, (smem));            \
     if (e_ != cudaSuccess) { err_expr; }                                                                         \
