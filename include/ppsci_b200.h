@@ -235,7 +235,13 @@ int ppsci_b200_residual_fwd(ppsci_plan* plan, const void* const* x_cols,
 int64_t ppsci_b200_plan_last_launches(const ppsci_plan* plan);
 
 /* Test accessor: byte offset inside the (256-aligned) workspace of the jet planes of `layer`
- * ([C][min(n_points, chunk)][round4(width)]); layer == n_layers addresses the output jets. */
+ * ([C][min(n_points, chunk)][round4(width)]); layer == n_layers addresses the output jets.
+ * layer == 300: the output adjoints Ybar (same layout as the output jets).
+ * layer == 301 / 302: the two ping-pong buffers of the hidden adjoints Zbar.  After an adjoint over L = n_layers
+ * layers, Zbar_l (l >= 1) was last written to buffer (L-1-l) mod 2 (301 for 0, 302 for 1), so only the two lowest,
+ * Zbar_1 and Zbar_2, survive the call.  Zbar_l is laid out [C][min(n_points, chunk)][round4(width_l)], plane pitch
+ * min(n_points, chunk) * round4(width_l).  After a multi-chunk call every buffer holds the last chunk.  The rule does
+ * not hold for gated networks (ModifiedMLP, PirateNet), whose gate kernels also work in these buffers. */
 int64_t ppsci_b200_plan_stash_offset(const ppsci_plan* plan, int64_t n_points, int32_t layer);
 
 /* Forward + adjoint of the network VALUES for caller-supplied output adjoints: runs the forward pass (stash), seeds

@@ -462,12 +462,15 @@ extern "C" int32_t ppsci_b200_plan_uses_tcgen05(const ppsci_plan* P) { return (P
 // Debug / test accessor: byte offset (from the 256-aligned workspace base) of the jet planes of
 // `layer` for a call with n_points points: layer in [1, n_layers) -> hidden pre-activations Z_l,
 // layer == n_layers -> output jets Y.  Layout [C][min(n_points, chunk)][ld], ld = round4(width).
+// 301 / 302 -> the Zbar ping-pong buffers zbar0 / zbar1 (the adjoint writes Zbar_l into buffer (L-1-l) mod 2).
 extern "C" int64_t ppsci_b200_plan_stash_offset(const ppsci_plan* P, int64_t n_points, int32_t layer) {
   if (!P || n_points <= 0) return -1;
   const int64_t nc = n_points < P->chunk ? n_points : P->chunk;
   Carve cv;
   carve(P, nc, &cv);
   if (layer == 300) return (int64_t)cv.ybar;  // output adjoints Ybar (values_bwd_kept accepts this address: no seeding copy)
+  if (layer == 301) return (int64_t)cv.zbar0;
+  if (layer == 302) return (int64_t)cv.zbar1;
   if (layer < 1 || layer > P->spec.n_layers) return -1;
   return (int64_t)(layer < P->spec.n_layers ? cv.z[layer] : cv.y);
 }

@@ -427,8 +427,16 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_layer(WgArgs g) {
 // (the 3xTF32 scheme of k_wg_layer, with the exact-product term in an accumulator of its own).  While the MMAs of chunk j
 // run, the Zbar_l values of chunk j + 1 are loaded into registers and written to the other B stage, and its Z_{l-1}
 // values are copied into per-thread shared-memory slots by cp.async (they would not fit in registers beside the two
-// accumulators and the in-flight A fragments); the jets are computed once those MMAs have retired.  The CTA flushes once
-// with atomicAdd; the CTAs of fan-in block 0 also add their columns' channel-0 sums (summed in shared memory) to db_l.
+// accumulators and the in-flight A fragments); the jets are computed once those MMAs have retired.  Every dw_flush(C)
+// chunks each thread adds its accumulators to partial sums of its own in shared memory (fp32, round to nearest) and
+// restarts them at zero.  The CTA adds partial sums and accumulators to dW_l once, with atomicAdd; the CTAs of fan-in
+// block 0 also add their columns' channel-0 sums (summed in shared memory) to db_l.
+//
+// Why the periodic flush: the tensor cores do not round each accumulation to nearest, so the error of a wgmma
+// accumulator grows linearly with the number of K steps added into it, not like a random walk.  Accumulated over a
+// whole split (up to ~10^5 jet rows at 70,001 points), dW_l was off by up to ~8,000 units of 2^-24 sum |A| |Zbar|
+// against ~50 for the CUDA-core kernel (measured on an H100 80GB HBM3, 700 W power limit; tests/test_gpu_tc_layers.py).
+// Restarting the accumulators every ~512 jet rows bounds that error independently of the point count.
 __host__ __device__ constexpr int dw_pch(int C) { return C >= 8 ? 4 : C >= 3 ? 8 : 32 / C; }  // points per chunk
 __host__ __device__ constexpr int dw_groups(int C) { return dw_pch(C) / 4 * C; }
 __host__ __device__ constexpr int dw_ksteps(int C) { return (dw_groups(C) + 1) / 2; }
@@ -437,12 +445,16 @@ __host__ __device__ constexpr int dw_atoms(int C) { return (dw_ksteps(C) + 3) / 
 // prefetch of a chunk, must fit in 255 registers without spilling
 __host__ __device__ constexpr int dw_maxq(int C) { return C <= 5 ? 4 : C <= 8 ? 2 : 1; }
 __host__ __device__ constexpr int dw_q(int C, int q) { return q < dw_maxq(C) ? q : dw_maxq(C); }
-// two stages of [hi | lo][atoms][BN rows x 128 bytes], 1024-byte aligned, then the db_l column sums and the A operand's
-// per-thread Z_{l-1} slots
+// two stages of [hi | lo][atoms][BN rows x 128 bytes], 1024-byte aligned, then the db_l column sums, the A operand's
+// per-thread Z_{l-1} slots and the per-thread partial sums of the flushed accumulators (BN / 2 per thread)
 __host__ __device__ constexpr int dw_smem_bytes(int C, int bnq) {
-  return 2 * 2 * dw_atoms(C) * bnq * 32 * 128 + bnq * 32 * 4 + dw_pch(C) / 4 * 2 * C * 256 * 4 + 1024;
+  return 2 * 2 * dw_atoms(C) * bnq * 32 * 128 + bnq * 32 * 4 + dw_pch(C) / 4 * 2 * C * 256 * 4 + bnq * 32 * 2 * 256 + 1024;
 }
 constexpr int DW_TK = 128;  // fan-in rows per CTA
+constexpr int DW_FLUSH_ROWS = 512;  // jet rows accumulated by the tensor cores between two flushes to dW_l
+__host__ __device__ constexpr int dw_flush(int C) {  // chunks per flush
+  return DW_FLUSH_ROWS / (dw_pch(C) * C) > 1 ? DW_FLUSH_ROWS / (dw_pch(C) * C) : 1;
+}
 
 struct WgDwArgs {
   AOperand<float> A;   // A_ACT over Z_{l-1}
@@ -538,6 +550,30 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_dw(WgDwArgs g) {
 #pragma unroll
   for (int i = 0; i < (TAIL ? 16 : 1); ++i) ext[i] = crt[i] = 0.f;
 
+  // element e of this thread's accumulator fragments (exact + cross term): e = 4 j + 2 h + b is row krow + 8 h, column
+  // 8 j + 2 t + b of the n8 block j
+  auto acc_at = [&](int e) -> float {
+    return e < 32 * NB ? ex[e >> 5][e & 31] + cr[e >> 5][e & 31] : ext[e - 32 * NB] + crt[e - 32 * NB];
+  };
+  // partial sums of the flushed accumulators: float4 q of this thread (elements 4 q .. 4 q + 3) at part[q THREADS + tid]
+  float4* part = reinterpret_cast<float4*>(base_ptr + 2 * STAGE + BN * 4 + QPC * 2 * CS * THREADS * 4);
+#pragma unroll
+  for (int q = 0; q < BN / 8; ++q) part[q * THREADS + tid] = make_float4(0.f, 0.f, 0.f, 0.f);
+  auto flush = [&]() {
+#pragma unroll
+    for (int q = 0; q < BN / 8; ++q) {
+      float4 p = part[q * THREADS + tid];
+      p.x += acc_at(4 * q); p.y += acc_at(4 * q + 1); p.z += acc_at(4 * q + 2); p.w += acc_at(4 * q + 3);
+      part[q * THREADS + tid] = p;
+    }
+#pragma unroll
+    for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) ex[nb][i] = cr[nb][i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (TAIL ? 16 : 1); ++i) ext[i] = crt[i] = 0.f;
+  };
+
   // Z_{l-1} at point 4 qq + t of the chunk, fan-in row krow + 8 h, channel c: thread-private slots, filled by cp.async
   // (zero past Np and Kdim) while the previous chunk's MMAs run
   float* za = reinterpret_cast<float*>(base_ptr + 2 * STAGE + BN * 4);
@@ -601,6 +637,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_dw(WgDwArgs g) {
       if (kb == 0 && gi % CS == 0) atomicAdd(bsum + n, (v.x + v.y) + (v.z + v.w));
     }
     wgmma_wait<0>();  // the MMAs of chunk ch - 1 have retired: the fragment registers are free
+    if (ch > ch_begin && (ch - ch_begin) % dw_flush(CS) == 0) flush();
     // activation jets of this thread's A elements (points past Np give finite jets of 0 against zero B values)
     asm volatile("cp.async.wait_group 0;" ::: "memory");
     float av[QPC][2][CS];
@@ -653,8 +690,6 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_dw(WgDwArgs g) {
     if (ch + 1 < ch_end) load_b(ch + 1);
   }
   wgmma_wait<0>();
-
-  // accumulator fragment: element 4 j + 2 h + b of the n8 block j is row krow + 8 h, column 8 j + 2 t + b
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int k = krow + 8 * h;
@@ -664,12 +699,9 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_dw(WgDwArgs g) {
     for (int j = 0; j < BN / 8; ++j) {
       if (n0 + 8 * j >= g.Nout) break;
       const int col = 8 * j + 2 * t;
-      const float e0 = j < 8 * NB ? ex[j >> 3][4 * (j & 7) + 2 * h] : ext[4 * (j - 8 * NB) + 2 * h];
-      const float e1 = j < 8 * NB ? ex[j >> 3][4 * (j & 7) + 2 * h + 1] : ext[4 * (j - 8 * NB) + 2 * h + 1];
-      const float c0 = j < 8 * NB ? cr[j >> 3][4 * (j & 7) + 2 * h] : crt[4 * (j - 8 * NB) + 2 * h];
-      const float c1 = j < 8 * NB ? cr[j >> 3][4 * (j & 7) + 2 * h + 1] : crt[4 * (j - 8 * NB) + 2 * h + 1];
-      atomicAdd(row + col, e0 + c0);
-      atomicAdd(row + col + 1, e1 + c1);
+      const float4 p = part[j * THREADS + tid];
+      atomicAdd(row + col, (h ? p.z : p.x) + acc_at(4 * j + 2 * h));
+      atomicAdd(row + col + 1, (h ? p.w : p.y) + acc_at(4 * j + 2 * h + 1));
     }
   }
   if (kb == 0) {

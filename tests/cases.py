@@ -280,9 +280,21 @@ def run_case(name, n: int, library=None, device="cpu", backend: int = 0, seed: i
     else:
         lerr = max(abs(float(loss[i]) - float(lo_[k])) / max(1e-30, abs(float(lo_[k]))) for i, k in enumerate(cr.names))
         rerr = max(float((d_res[k].cpu().double() - ro[k]).norm() / ro[k].norm().clamp_min(1e-30)) for k in cr.names)
-        gerr = float((d_grads.cpu().double() - go).norm() / go.norm())
+        g = d_grads.cpu().double()
+        gerr = float((g - go).norm() / go.norm())
+        # per parameter block: an error confined to one layer's weights or bias is not diluted by the others
+        gblk, off = 0.0, 0
+        for a, b in zip(om.widths[:-1], om.widths[1:]):
+            for sl in (slice(off, off + a * b), slice(off + a * b, off + a * b + b)):
+                gblk = max(gblk, float((g[sl] - go[sl]).norm() / go[sl].norm().clamp_min(1e-30)))
+            off += a * b + b
+    # largest per-point residual error, in units of the residual's rms (an error confined to a few points shows)
+    rpt = max(float((d_res[k].cpu().double()[sub if sub is not None else slice(None)] - ro[k]).abs().max()
+                    / ro[k].pow(2).mean().sqrt().clamp_min(1e-30)) for k in cr.names)
+    if sub is not None:
+        gblk = float("nan")
     # forward-only entry point must agree with the fused call
     _, res2 = plan.forward(d_in, d_par, want_jets=False)
     ferr = max(float((res2[k] - d_res[k]).abs().max()) for k in cr.names)
-    return dict(loss=lerr, res=rerr, grad=gerr, fwd_vs_fused=ferr, channels=cr.channels, launches=plan.last_launches,
-                tc=plan.uses_tcgen05)
+    return dict(loss=lerr, res=rerr, grad=gerr, grad_block=gblk, res_point=rpt, fwd_vs_fused=ferr, channels=cr.channels,
+                launches=plan.last_launches, tc=plan.uses_tcgen05)

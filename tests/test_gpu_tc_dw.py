@@ -5,7 +5,7 @@ import pytest
 import torch
 
 from tests.cases import TC_CASES, run_case
-from tests.test_gpu_tc import TOL_TC
+from tests.test_gpu_tc import assert_tc
 
 pytestmark = pytest.mark.gpu
 
@@ -17,7 +17,5 @@ def test_tc_dw_uneven_blocks(mask, monkeypatch):
     assert torch.cuda.is_available()
     monkeypatch.setenv("PPSCI_B200_TC_MASK", str(mask))
     r = run_case(CASE, 3000, device="cuda:0", backend=2)
-    assert r["tc"], "tensor-core backend was not selected"
-    assert r["loss"] <= TOL_TC["loss"], r
-    assert r["res"] <= TOL_TC["res"], r
-    assert r["grad"] <= TOL_TC["grad"], r
+    print(f"[tc] dw_uneven mask={mask} {r}")
+    assert_tc(r)
