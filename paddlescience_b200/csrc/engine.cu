@@ -56,8 +56,22 @@ struct ppsci_plan {
   int chunk = 0;
   int num_sms = 132;
   bool use_wg = false;  // forward, dx and dW run on the wgmma kernels where the layer shapes allow (kernels_wgmma.cuh)
-  // PPSCI_B200_TC_MASK (cross-checks): bit 0 forward, bit 1 dx, bit 2 dW of the eligible layers on the tensor cores
-  int tc_mask = 255;
+  // PPSCI_B200_TC_MASK (cross-checks): bit 0 forward, bit 1 dx, bit 2 dW of the eligible layers on the tensor cores;
+  // the other bits are ignored
+  int tc_mask = 7;
+  // layer l's forward / dx / dW runs on the wgmma kernels; its forward (transposed) tf32 hi / lo weight image sits at
+  // img_off[l] (imgT_off[l]) of the wimg workspace region, img_bytes long in all
+  bool wg_fwd[PPSCI_MAX_LAYERS + 1] = {};
+  bool wg_dx[PPSCI_MAX_LAYERS + 1] = {};
+  bool wg_dw[PPSCI_MAX_LAYERS + 1] = {};
+  size_t img_off[PPSCI_MAX_LAYERS + 1] = {};
+  size_t imgT_off[PPSCI_MAX_LAYERS + 1] = {};
+  size_t img_bytes = 0;
+  // first / last layer on the thin kernels (kernels_thin.cuh); thin_vec: the vectorised ones, jet layout thin_lay
+  bool thin_first = false;
+  bool thin_last = false;
+  bool thin_vec = false;
+  int thin_lay = 0;
   // device copies of the residual program
   int* d_prog = nullptr;
   double* d_consts = nullptr;
@@ -119,46 +133,9 @@ struct Carve {
 // first gated layer (PirateNet always; ModifiedMLP with a Fourier embedding, act_first >= 0), 0 when they read the seeds
 static inline int gate_emb(const ppsci_plan_spec& s) { return (s.gated == 2 || (s.gated == 1 && s.act_first >= 0)) ? 1 : 0; }
 
-static inline int act_of_layer(const ppsci_plan_spec& s, int lin);
-// layer l's forward (dx) runs on the wgmma kernel; its weight image sits at wg_img_offset (wg_imgT_offset) of the wimg
-// region: the forward images first, then the transposed ones
-static bool wg_layer(const ppsci_plan* P, int l) {
-#ifdef PPSCI_EMUL
-  (void)P; (void)l;
-  return false;
-#else
-  return P->use_wg && (P->tc_mask & 1) && wg_fwd_ok(P->spec, l, P->J);
-#endif
-}
-static bool wg_dx_layer(const ppsci_plan* P, int l) {
-#ifdef PPSCI_EMUL
-  (void)P; (void)l;
-  return false;
-#else
-  return P->use_wg && (P->tc_mask & 2) && wg_dx_ok(P->spec, l, P->J);
-#endif
-}
-static bool wg_dw_layer(const ppsci_plan* P, int l) {
-#ifdef PPSCI_EMUL
-  (void)P; (void)l;
-  return false;
-#else
-  return P->use_wg && (P->tc_mask & 4) && wg_dw_ok(P->spec, l, P->J);
-#endif
-}
-static size_t wg_img_offset(const ppsci_plan* P, int layer) {
-  size_t off = 0;
-  for (int l = 1; l < layer; ++l)  // layer 1: a dense first layer, contraction padded to the chunk width
-    if (wg_layer(P, l))
-      off += (size_t)(l == 1 ? (P->spec.widths[0] + 31) / 32 * 32 : P->spec.widths[l - 1]) * P->spec.widths[l] * 8;
-  return off;
-}
-static size_t wg_imgT_offset(const ppsci_plan* P, int layer) {
-  size_t off = wg_img_offset(P, P->spec.n_layers + 1);
-  for (int l = 2; l < layer; ++l)
-    if (wg_dx_layer(P, l)) off += (size_t)P->spec.widths[l - 1] * P->spec.widths[l] * 8;
-  return off;
-}
+// activation applied to the output of linear layer `lin` (1-based)
+static inline int act_of_layer(const ppsci_plan_spec& s, int lin) { return (lin == 1 && s.act_first >= 0) ? s.act_first : s.act; }
+static inline bool act_has_param(int act) { return act == PPSCI_ACT_STAN || act == PPSCI_ACT_SWISH_B; }
 
 static void carve(const ppsci_plan* P, int64_t nc, Carve* cv) {
   const size_t es = P->spec.dtype == PPSCI_F64 ? 8 : 4;
@@ -176,7 +153,7 @@ static void carve(const ppsci_plan* P, int64_t nc, Carve* cv) {
   cv->zbar1 = take((size_t)P->C * nc * P->ld_hidden_max * es);
   for (int l = 2; l <= L; ++l) cv->wt[l] = take((size_t)P->spec.widths[l] * P->spec.widths[l - 1] * es);
   cv->loss_acc = take(PPSCI_MAX_RES * sizeof(double));
-  cv->wimg = take(wg_imgT_offset(P, L + 1));
+  cv->wimg = take(P->img_bytes);
   const bool gated = P->spec.gated != 0;
   for (int l = 1; l < L; ++l) cv->gt[l] = take(gated ? (size_t)P->C * nc * P->ld[l] * es : 0);
   const int emb = gate_emb(P->spec);
@@ -387,7 +364,25 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
     if (((P->tc_mask & 1) && wg_fwd_ok(*s, l, P->J)) || ((P->tc_mask & 2) && wg_dx_ok(*s, l, P->J)) ||
         ((P->tc_mask & 4) && wg_dw_ok(*s, l, P->J)))
       P->use_wg = true;
+  for (int l = 1; l <= s->n_layers && P->use_wg; ++l) {  // use_wg also gates a dense first layer
+    P->wg_fwd[l] = (P->tc_mask & 1) && wg_fwd_ok(*s, l, P->J);
+    P->wg_dx[l] = (P->tc_mask & 2) && wg_dx_ok(*s, l, P->J);
+    P->wg_dw[l] = (P->tc_mask & 4) && wg_dw_ok(*s, l, P->J);
+  }
 #endif
+  for (int l = 1; l <= s->n_layers; ++l) {  // the forward images first; layer 1: contraction padded to the chunk width
+    P->img_off[l] = P->img_bytes;
+    if (P->wg_fwd[l]) P->img_bytes += (size_t)(l == 1 ? (s->widths[0] + 31) / 32 * 32 : s->widths[l - 1]) * s->widths[l] * 8;
+  }
+  for (int l = 1; l <= s->n_layers; ++l) {
+    P->imgT_off[l] = P->img_bytes;
+    if (P->wg_dx[l]) P->img_bytes += (size_t)s->widths[l - 1] * s->widths[l] * 8;
+  }
+  const bool thin_on = getenv("PPSCI_B200_NO_THIN") == nullptr;
+  P->thin_first = thin_on && s->n_layers >= 2 && s->widths[0] <= THIN_MAXF && !s->dense_in && !s->gated;
+  P->thin_last = thin_on && s->n_layers >= 2 && n_out <= THIN_MAXM && C * n_out <= THIN_MAXCM && !s->gated && !act_has_param(s->act);
+  P->thin_lay = pick_layout(P->J, PPSCI_ACT_TANH);
+  P->thin_vec = s->dtype == PPSCI_F32 && P->thin_lay != LAY_DYN && getenv("PPSCI_B200_NO_THINV") == nullptr;
   if (s->backend == 2 && !P->use_wg) {
     delete P;
     return fail("plan_create: backend=2 (tensor cores) requested but the plan is not eligible (needs f32, hidden widths that "
@@ -485,27 +480,6 @@ extern "C" size_t ppsci_b200_plan_workspace_bytes(const ppsci_plan* P, int64_t n
 
 // ---------------------------------------------------------------------------------------------
 template <typename T>
-struct Dims {
-  static constexpr int TN = sizeof(T) == 8 ? 64 : 128;
-};
-
-template <typename T, int KMAX>
-static int set_attrs_once(ppsci_plan* P) {
-  constexpr int TN = Dims<T>::TN;
-  auto kf = k_gemm_fwd<T, TN, KMAX>;
-  auto kx = k_gemm_dx<T, TN, KMAX>;
-  auto kw = k_gemm_dw<T, TN, KMAX>;
-  const int smem_f = (KC * TMS + KC * TN) * (int)sizeof(T);
-  const int smem_x = std::max(smem_f, TM * TN * (int)sizeof(T));
-  const int smem_w = (RC * TMS + RC * TN) * (int)sizeof(T);
-  CK(cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_f));
-  CK(cudaFuncSetAttribute(kx, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_x));
-  CK(cudaFuncSetAttribute(kw, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_w));
-  (void)P;
-  return 0;
-}
-
-template <typename T>
 static void fill_seed(const ppsci_plan* P, const void* const* x_cols, int64_t x_off, AOperand<T>* A) {
   const ppsci_plan_spec& s = P->spec;
   A->mode = A_SEED;
@@ -526,10 +500,6 @@ static void fill_seed(const ppsci_plan* P, const void* const* x_cols, int64_t x_
     for (int i = 0; i < PPSCI_MAX_IN; ++i) S.dir_vec[d][i] = (d < s.n_dir && i < s.n_in) ? s.dir_vec[d][i] : 0.0;
   for (int i = 0; i < PPSCI_MAX_IN; ++i) S.x_cols[i] = i < s.n_in ? x_cols[i] : nullptr;
 }
-
-// activation applied to the output of linear layer `lin` (1-based)
-static inline int act_of_layer(const ppsci_plan_spec& s, int lin) { return (lin == 1 && s.act_first >= 0) ? s.act_first : s.act; }
-static inline bool act_has_param(int act) { return act == PPSCI_ACT_STAN || act == PPSCI_ACT_SWISH_B; }
 
 template <typename T>
 static void fill_act(const ppsci_plan* P, const T* Z, int ld, int64_t nc, int mode, AOperand<T>* A, int lin = 0) {
@@ -574,15 +544,34 @@ struct CallArgs {
   int phase = 0;                  // 0: forward + adjoint; 1: forward only, stash kept for a later adjoint; 2: adjoint from the kept stash
 };
 
+// split of a dW GEMM along the points: `want` splits, clamped to [1, total_chunks], of chunks_per_split chunks each
+struct DwSplit {
+  int chunks_per_split;
+  unsigned splits;
+};
+static DwSplit dw_split(long long want, long long total_chunks) {
+  want = std::min(std::max(want, 1LL), total_chunks);
+  const long long cps = (total_chunks + want - 1) / want;
+  return {(int)cps, (unsigned)((total_chunks + cps - 1) / cps)};
+}
+
 template <typename T, int KMAX>
 static int run(ppsci_plan* P, const CallArgs& a) {
-  constexpr int TN = Dims<T>::TN;
+  constexpr int TN = sizeof(T) == 8 ? 64 : 128;
   const ppsci_plan_spec& s = P->spec;
   const int L = s.n_layers;
   const int C = P->C;
   const int n_out = s.widths[L];
+  auto kf = k_gemm_fwd<T, TN, KMAX>;
+  auto kx = k_gemm_dx<T, TN, KMAX>;
+  auto kw = k_gemm_dw<T, TN, KMAX>;
+  const int smem_f = (KC * TMS + KC * TN) * (int)sizeof(T);
+  const int smem_x = std::max(smem_f, TM * TN * (int)sizeof(T));
+  const int smem_w = (RC * TMS + RC * TN) * (int)sizeof(T);
   if (!P->attrs_set) {
-    if (set_attrs_once<T, KMAX>(P)) return 1;
+    CK(cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_f));
+    CK(cudaFuncSetAttribute(kx, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_x));
+    CK(cudaFuncSetAttribute(kw, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_w));
     P->attrs_set = true;
   }
   const int64_t nc_max = a.n_points < P->chunk ? a.n_points : P->chunk;
@@ -600,31 +589,19 @@ static int run(ppsci_plan* P, const CallArgs& a) {
   P->ev_used = 0;
   P->ev_cls.clear();
 
-  auto kf = k_gemm_fwd<T, TN, KMAX>;
-  auto kx = k_gemm_dx<T, TN, KMAX>;
-  auto kw = k_gemm_dw<T, TN, KMAX>;
-  const int smem_f = (KC * TMS + KC * TN) * (int)sizeof(T);
-  const int smem_x = std::max(smem_f, TM * TN * (int)sizeof(T));
-  const int smem_w = (RC * TMS + RC * TN) * (int)sizeof(T);
+  // every launch of a call: timed in class cls when profiling, counted by plan_last_launches
+  auto launch = [&](int cls, auto kernel, dim3 grid, dim3 block, int smem, auto... args) {
+    ProfScope ps_(P, cls, st);
+    PPSCI_LAUNCH(kernel, grid, block, smem, st, args...);
+    P->launches++;
+  };
+  // Zbar_l: Ybar for l == L, otherwise ping-pong buffer (L - 1 - l) mod 2 (include/ppsci_b200.h)
+  auto zbar = [&](int l) { return reinterpret_cast<T*>(ws + (l == L ? cv.ybar : (L - 1 - l) % 2 ? cv.zbar1 : cv.zbar0)); };
   const int TP = TM / C;
   const int PT = RC / C;
-  const bool thin_on = getenv("PPSCI_B200_NO_THIN") == nullptr;
   const bool gated = s.gated != 0;  // ModifiedMLP: generic tile GEMMs + the gate kernels (kernels_gate.cuh)
-  const bool thin_first = thin_on && L >= 2 && s.widths[0] <= THIN_MAXF && !s.dense_in && !gated;
-  const bool thin_last = thin_on && L >= 2 && n_out <= THIN_MAXM && C * n_out <= THIN_MAXCM && !gated && !act_has_param(s.act);
-  // A_ACT operand of layer lin + 1: beta(s) of layer lin's activation
-  auto set_actp = [&](AOperand<T>* A, int lin) {
-    if (lin >= 1 && lin < L && P->actp_off[lin] >= 0) {
-      A->act_param = params + P->actp_off[lin];
-      A->act_pstride = P->actp_stride;
-    }
-  };
   if (gated && a.phase != 0) return fail("two-phase value calls are not offered for gated networks");
   const bool pirate = s.gated == 2;  // PirateNet: layer 1 = embedding, blocks of (gate, gate, adaptive residual)
-  auto kgf = k_gate_fwd<T, KMAX>;
-  auto kgb = k_gate_bwd<T, KMAX>;
-  auto kmf = k_mix_fwd<T, KMAX>;
-  auto kmb = k_mix_bwd<T, KMAX>;
   // what follows hidden layer l in a gated plan: 0 gate, 1 adaptive residual (end of a block), 2 plain activation
   const int emb = gated ? gate_emb(s) : 0;  // layer 1 is an embedding layer (its stored output feeds embed_u / embed_v)
   auto post_kind = [&](int l) -> int { return (emb && l == 1) ? 2 : ((pirate && (l - 2) % 3 == 2) ? 1 : 0); };
@@ -654,9 +631,43 @@ static int run(ppsci_plan* P, const CallArgs& a) {
     ga->Np = nc;
     ga->H = s.widths[l];
   };
-  // fp32 + one of the compile-time jet layouts: vectorised thin kernels (kernels_thin.cuh)
-  const int thin_lay = pick_layout(P->J, PPSCI_ACT_TANH);
-  const bool thin_vec = sizeof(T) == 4 && thin_lay != LAY_DYN && getenv("PPSCI_B200_NO_THINV") == nullptr;
+  // A operand of linear layer l for the chunk at point c0: the network input (layer 1), the stored output G_{l-1} of
+  // what follows layer l-1 in a gated plan, or act(Z_{l-1}) with the activation's trainable parameter if it has one
+  auto operand = [&](int l, int64_t c0) {
+    AOperand<T> A;
+    memset(&A, 0, sizeof(A));
+    if (l == 1) {
+      fill_first<T>(P, a.x_cols, c0, nc_max, &A);
+    } else if (gated) {
+      fill_act<T>(P, reinterpret_cast<const T*>(ws + cv.gt[l - 1]), P->ld[l - 1], nc_max, A_PLAIN, &A);
+    } else {
+      fill_act<T>(P, reinterpret_cast<const T*>(ws + cv.z[l - 1]), P->ld[l - 1], nc_max, A_ACT, &A, l - 1);
+      if (P->actp_off[l - 1] >= 0) {
+        A.act_param = params + P->actp_off[l - 1];
+        A.act_pstride = P->actp_stride;
+      }
+    }
+    return A;
+  };
+#ifndef PPSCI_EMUL
+  // k_wg_layer over a chunk of nc points (dx: Zbar_{l-1} from Zbar_l) with the weight image at img_off of the wimg
+  // region, output in the pitch of layer lo; a persistent grid of at most one CTA per SM
+  auto launch_wg = [&](int cls, bool dx, wg::WgArgs& w, size_t img_off, int lo, float* out, int64_t nc) -> int {
+    w.J = P->J;
+    w.Wimg = reinterpret_cast<const float*>(ws + cv.wimg + img_off);
+    w.Out = out;
+    w.ldo = P->ld[lo];
+    w.oplane = (long long)nc_max * P->ld[lo];
+    w.Np = nc;
+    const unsigned tiles = (unsigned)((nc + wg::tile_points(C) - 1) / wg::tile_points(C));
+    w.num_tiles = (int)tiles;
+    const int smem = wg::fwd_smem_bytes(w.Nout);
+    const auto k = dx ? wg_layer_kernel<true>(wg_layout(P->J), w.Nout) : wg_layer_kernel<false>(wg_layout(P->J), w.Nout);
+    CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    launch(cls, k, dim3(tiles < (unsigned)P->num_sms ? tiles : (unsigned)P->num_sms), dim3(wg::THREADS), smem, w);
+    return 0;
+  };
+#endif
 
   if (a.want_loss) CK(cudaMemsetAsync(loss_acc, 0, PPSCI_MAX_RES * sizeof(double), st));
   // phase 1 runs the forward exactly as a training call would (stash of everything the adjoint reads), phase 2 only the adjoint
@@ -664,46 +675,35 @@ static int run(ppsci_plan* P, const CallArgs& a) {
   if (a.phase == 2 && a.n_points > nc_max)
     return fail("values_bwd_kept: the kept stash covers one workspace chunk (" + std::to_string(nc_max) + " points); got " +
                 std::to_string(a.n_points));
-  if (do_bwd) {
-    for (int l = 2; l <= L; ++l) {
-      const int K = s.widths[l - 1], N = s.widths[l];
-      const long long tot = (long long)K * N;
-      auto kt = k_transpose<T>;
-      ProfScope ps_(P, CLS_MISC, st);
-      PPSCI_LAUNCH(kt, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st, params + P->w_off[l],
-                   reinterpret_cast<T*>(ws + cv.wt[l]), K, N);
-      P->launches++;
-    }
-    for (int e = 0; e < (emb ? 2 : 0); ++e) {  // the embeddings hand an adjoint back to layer 1's output
-      const int K = s.widths[1], N = s.widths[2];
-      const long long tot = (long long)K * N;
-      auto kt = k_transpose<T>;
-      ProfScope ps_(P, CLS_MISC, st);
-      PPSCI_LAUNCH(kt, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st, params + P->gate_w_off[e],
-                   reinterpret_cast<T*>(ws + (e == 0 ? cv.wtu : cv.wtv)), K, N);
-      P->launches++;
+  if (do_bwd) {  // W_l^T for l >= 2; the embeddings hand an adjoint back to layer 1's output: Wu^T, Wv^T (layer 2's shape)
+    struct Transpose {
+      int l;       // layer whose shape the weights have
+      int64_t w;   // weights in params
+      size_t wt;   // transpose in the workspace
+    };
+    std::vector<Transpose> tr;
+    for (int l = 2; l <= L; ++l) tr.push_back({l, P->w_off[l], cv.wt[l]});
+    for (int e = 0; e < (emb ? 2 : 0); ++e) tr.push_back({2, P->gate_w_off[e], e == 0 ? cv.wtu : cv.wtv});
+    for (const Transpose& t : tr) {
+      const int K = s.widths[t.l - 1], N = s.widths[t.l];
+      launch(CLS_MISC, k_transpose<T>, dim3((unsigned)(((long long)K * N + 255) / 256)), dim3(256), 0, params + t.w,
+             reinterpret_cast<T*>(ws + t.wt), K, N);
     }
   }
 
 #ifndef PPSCI_EMUL
   for (int l = 1; l <= L; ++l) {  // tf32 hi / lo images of the weights of the wgmma-served layers, once per call
-    const long long tot = (long long)s.widths[l - 1] * s.widths[l];
-    if (wg_layer(P, l) && a.phase != 2) {
-      ProfScope ps_(P, CLS_MISC, st);
+    const dim3 grid((unsigned)(((long long)s.widths[l - 1] * s.widths[l] + 255) / 256));
+    const float* W = reinterpret_cast<const float*>(params) + P->w_off[l];
+    if (P->wg_fwd[l] && a.phase != 2) {
       if (l == 1)  // zero rows beyond the dense first layer's contraction length
-        CK(cudaMemsetAsync(ws + cv.wimg + wg_img_offset(P, 1), 0, (size_t)wg_kpad(s.widths[0]) * s.widths[1] * 8, st));
-      PPSCI_LAUNCH(wg::k_wg_prep_w, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st,
-                   reinterpret_cast<const float*>(params) + P->w_off[l], reinterpret_cast<float*>(ws + cv.wimg + wg_img_offset(P, l)),
-                   s.widths[l - 1], s.widths[l], 0);
-      P->launches++;
+        CK(cudaMemsetAsync(ws + cv.wimg + P->img_off[1], 0, (size_t)wg_kpad(s.widths[0]) * s.widths[1] * 8, st));
+      launch(CLS_MISC, wg::k_wg_prep_w, grid, dim3(256), 0, W, reinterpret_cast<float*>(ws + cv.wimg + P->img_off[l]),
+             s.widths[l - 1], s.widths[l], 0);
     }
-    if (wg_dx_layer(P, l) && do_bwd) {  // gemm K = fan-out, gemm N = fan-in
-      ProfScope ps_(P, CLS_MISC, st);
-      PPSCI_LAUNCH(wg::k_wg_prep_w, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st,
-                   reinterpret_cast<const float*>(params) + P->w_off[l], reinterpret_cast<float*>(ws + cv.wimg + wg_imgT_offset(P, l)),
-                   s.widths[l], s.widths[l - 1], 1);
-      P->launches++;
-    }
+    if (P->wg_dx[l] && do_bwd)  // gemm K = fan-out, gemm N = fan-in
+      launch(CLS_MISC, wg::k_wg_prep_w, grid, dim3(256), 0, W, reinterpret_cast<float*>(ws + cv.wimg + P->imgT_off[l]),
+             s.widths[l], s.widths[l - 1], 1);
   }
 #endif
   for (int64_t c0 = 0; c0 < a.n_points; c0 += nc_max) {
@@ -711,40 +711,34 @@ static int run(ppsci_plan* P, const CallArgs& a) {
     const unsigned ptiles = (unsigned)((nc + TP - 1) / TP);
     // ---------------- forward ----------------
     for (int l = (a.phase == 2 ? L + 1 : 1); l <= L; ++l) {
-      if (l == 1 && thin_first) {
+      if (l == 1 && P->thin_first) {
         FirstArgs<T> f;
         memset(&f, 0, sizeof(f));
-        fill_seed<T>(P, a.x_cols, c0, &f.A);
+        f.A = operand(1, c0);
         f.J = P->J;
         f.W = params + P->w_off[1];
         f.bias = params + P->b_off[1];
         f.nf = s.widths[0];
         f.N = s.widths[1];
-        f.Out = reinterpret_cast<T*>(ws + (L > 1 ? cv.z[1] : cv.y));
+        f.Out = reinterpret_cast<T*>(ws + cv.z[1]);
         f.ldo = P->ld[1];
         f.oplane = (long long)nc_max * P->ld[1];
         f.Np = nc;
-        const long long tot = (long long)nc * f.N;
+        void (*k)(FirstArgs<T>) = k_first_fwd<T, KMAX>;
+        dim3 grid((unsigned)((nc * f.N + 255) / 256));
         if constexpr (sizeof(T) == 4) {
-          if (thin_vec && f.N % 4 == 0) {  // compile-time layout, 128-bit stores, seeds staged once per point
-            void (*kv)(FirstArgs<float>) = nullptr;
-            PPSCI_THIN_PICK_L(k_first_fwd_v, thin_lay, KMAX, kv);
-            ProfScope ps_(P, CLS_THIN_FWD, st);
-            PPSCI_LAUNCH(kv, dim3((unsigned)((nc + thin::PB - 1) / thin::PB)), dim3(256), 0, st, f);
-            P->launches++;
-            continue;
+          if (P->thin_vec && f.N % 4 == 0) {  // compile-time layout, 128-bit stores, seeds staged once per point
+            PPSCI_THIN_PICK_L(k_first_fwd_v, P->thin_lay, KMAX, k);
+            grid = dim3((unsigned)((nc + thin::PB - 1) / thin::PB));
           }
         }
-        auto k1 = k_first_fwd<T, KMAX>;
-        ProfScope ps_(P, CLS_THIN_FWD, st);
-        PPSCI_LAUNCH(k1, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st, f);
-        P->launches++;
+        launch(CLS_THIN_FWD, k, grid, dim3(256), 0, f);
         continue;
       }
-      if (l == L && thin_last) {
+      if (l == L && P->thin_last) {
         LastArgs<T> f;
         memset(&f, 0, sizeof(f));
-        fill_act<T>(P, reinterpret_cast<const T*>(ws + cv.z[L - 1]), P->ld[L - 1], nc_max, A_ACT, &f.A, L - 1);
+        f.A = operand(L, c0);
         f.J = P->J;
         f.W = params + P->w_off[L];
         f.bias = params + P->b_off[L];
@@ -754,64 +748,36 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         f.ldy = P->ld[L];
         f.yplane = (long long)nc_max * P->ld[L];
         f.Np = nc;
+        void (*k)(LastArgs<T>) = k_last_fwd<T, KMAX>;
         if constexpr (sizeof(T) == 4) {
-          if (thin_vec && f.K % 4 == 0 && f.m <= 4) {
-            void (*kv)(LastArgs<float>) = nullptr;
-            PPSCI_THIN_PICK_LM(k_last_fwd_v, thin_lay, f.m, kv);
-            ProfScope ps_(P, CLS_THIN_FWD, st);
-            PPSCI_LAUNCH(kv, dim3((unsigned)((nc + 7) / 8)), dim3(256), 0, st, f);
-            P->launches++;
-            continue;
-          }
+          if (P->thin_vec && f.K % 4 == 0 && f.m <= 4) PPSCI_THIN_PICK_LM(k_last_fwd_v, P->thin_lay, f.m, k);
         }
-        auto k2 = k_last_fwd<T, KMAX>;
-        ProfScope ps_(P, CLS_THIN_FWD, st);
-        PPSCI_LAUNCH(k2, dim3((unsigned)((nc + 7) / 8)), dim3(256), 0, st, f);
-        P->launches++;
+        launch(CLS_THIN_FWD, k, dim3((unsigned)((nc + 7) / 8)), dim3(256), 0, f);
         continue;
       }
 #ifndef PPSCI_EMUL
-      if (sizeof(T) == 4 && wg_layer(P, l)) {
-        wg::WgArgs w;
-        memset(&w, 0, sizeof(w));
-        w.Kdim = s.widths[l - 1];
-        if (l == 1) {  // dense first layer: the caller's [n_points][n_feat] matrix as is, columns beyond n_feat read as zero
-          const int nf = s.widths[0];
-          fill_act<float>(P, reinterpret_cast<const float*>(a.x_cols[0]) + c0 * nf, nf, nc_max, A_ACT, &w.A);
-          w.A.act = PPSCI_ACT_IDENTITY;
-          w.Kdim = wg_kpad(nf);
-          w.Kvalid = nf;
-        } else {
-          fill_act<float>(P, reinterpret_cast<const float*>(ws + cv.z[l - 1]), P->ld[l - 1], nc_max, A_ACT, &w.A, l - 1);
+      if (P->wg_fwd[l]) {
+        if constexpr (sizeof(T) == 4) {
+          wg::WgArgs w;
+          memset(&w, 0, sizeof(w));
+          w.A = operand(l, c0);
+          w.Kdim = s.widths[l - 1];
+          if (l == 1) {  // dense first layer: the caller's [n_points][n_feat] matrix as is, columns beyond n_feat read as zero
+            w.A.act = PPSCI_ACT_IDENTITY;
+            w.Kdim = wg_kpad(s.widths[0]);
+            w.Kvalid = s.widths[0];
+          }
+          w.Nout = s.widths[l];
+          w.bias = params + P->b_off[l];
+          // a wide output layer writes Y
+          if (launch_wg(CLS_FWD, false, w, P->img_off[l], l, reinterpret_cast<T*>(ws + (l < L ? cv.z[l] : cv.y)), nc)) return 1;
         }
-        w.J = P->J;
-        w.Wimg = reinterpret_cast<const float*>(ws + cv.wimg + wg_img_offset(P, l));
-        w.Nout = s.widths[l];
-        w.bias = reinterpret_cast<const float*>(params) + P->b_off[l];
-        w.Out = reinterpret_cast<float*>(ws + (l < L ? cv.z[l] : cv.y));  // a wide output layer writes Y
-        w.ldo = P->ld[l];
-        w.oplane = (long long)nc_max * P->ld[l];
-        w.Np = nc;
-        const unsigned wtiles = (unsigned)((nc + wg::tile_points(C) - 1) / wg::tile_points(C));
-        w.num_tiles = (int)wtiles;
-        const int smem = wg::fwd_smem_bytes(w.Nout);
-        const unsigned gridx = wtiles < (unsigned)P->num_sms ? wtiles : (unsigned)P->num_sms;
-        ProfScope ps_(P, CLS_FWD, st);
-        PPSCI_WG_LAUNCH(false, wg_layout(P->J), w.Nout, dim3(gridx), smem, st, w,
-                        return fail(std::string("cudaFuncSetAttribute(k_wg_layer): ") + cudaGetErrorString(e_)));
-        P->launches++;
         continue;
       }
 #endif
       GemmArgs<T> g;
       memset(&g, 0, sizeof(g));
-      if (l == 1) fill_first<T>(P, a.x_cols, c0, nc_max, &g.A);
-      else if (gated)  // the gate / residual / activation that follows layer l-1 was stored when that layer finished
-        fill_act<T>(P, reinterpret_cast<const T*>(ws + cv.gt[l - 1]), P->ld[l - 1], nc_max, A_PLAIN, &g.A);
-      else {
-        fill_act<T>(P, reinterpret_cast<const T*>(ws + cv.z[l - 1]), P->ld[l - 1], nc_max, A_ACT, &g.A, l - 1);
-        set_actp(&g.A, l - 1);
-      }
+      g.A = operand(l, c0);
       g.J = P->J;
       g.B = params + P->w_off[l];
       g.Kdim = s.widths[l - 1];
@@ -823,47 +789,34 @@ static int run(ppsci_plan* P, const CallArgs& a) {
       g.oplane = (long long)nc_max * P->ld[l];
       g.Np = nc;
       g.TP = TP;
-      dim3 grid(ptiles, (unsigned)((g.Nout + TN - 1) / TN));
-      {
-        ProfScope ps_(P, CLS_FWD, st);
-        PPSCI_LAUNCH(kf, grid, dim3(NTHREADS), smem_f, st, g);
-        P->launches++;
-      }
+      launch(CLS_FWD, kf, dim3(ptiles, (unsigned)((g.Nout + TN - 1) / TN)), dim3(NTHREADS), smem_f, g);
       auto post_fwd = [&](int lay) {  // operand of layer lay + 1
-        const long long tot = (long long)nc * s.widths[lay];
-        ProfScope ps_(P, CLS_MISC, st);
+        const dim3 grid((unsigned)(((long long)nc * s.widths[lay] + 127) / 128));
         if (post_kind(lay) == 0) {  // G = V + act(Z) (U - V)
           GateArgs<T> ga;
           fill_gate(lay, nc, &ga);
           ga.G = reinterpret_cast<T*>(ws + cv.gt[lay]);
-          PPSCI_LAUNCH(kgf, dim3((unsigned)((tot + 127) / 128)), dim3(128), 0, st, ga);
+          launch(CLS_MISC, k_gate_fwd<T, KMAX>, grid, dim3(128), 0, ga);
         } else {  // X = alpha act(Z) + (1 - alpha) X_block_in, or X = act(Z)
           MixArgs<T> ma;
           fill_mix(lay, nc, &ma);
           ma.X = reinterpret_cast<T*>(ws + cv.gt[lay]);
-          PPSCI_LAUNCH(kmf, dim3((unsigned)((tot + 127) / 128)), dim3(128), 0, st, ma);
+          launch(CLS_MISC, k_mix_fwd<T, KMAX>, grid, dim3(128), 0, ma);
         }
-        P->launches++;
       };
       if (emb && l == 1) post_fwd(1);
       if (gated && l == 1) {  // embed_u / embed_v: two more layers from the seeds, or from the embedding layer's output
-        dim3 grid_e = grid;
-        if (emb) {
-          fill_act<T>(P, reinterpret_cast<const T*>(ws + cv.gt[1]), P->ld[1], nc_max, A_PLAIN, &g.A);
-          g.Kdim = s.widths[1];
-          g.Nout = s.widths[2];
-          g.ldb = s.widths[2];
-          g.ldo = P->ld[2];
-          g.oplane = (long long)nc_max * P->ld[2];
-          grid_e = dim3(ptiles, (unsigned)((g.Nout + TN - 1) / TN));
-        }
+        g.A = operand(emb + 1, c0);
+        g.Kdim = s.widths[emb];
+        g.Nout = s.widths[emb + 1];
+        g.ldb = s.widths[emb + 1];
+        g.ldo = P->ld[emb + 1];
+        g.oplane = (long long)nc_max * P->ld[emb + 1];
         for (int e = 0; e < 2; ++e) {
           g.B = params + P->gate_w_off[e];
           g.bias = params + P->gate_b_off[e];
           g.Out = reinterpret_cast<T*>(ws + (e == 0 ? cv.zu : cv.zv));
-          ProfScope ps_(P, CLS_FWD, st);
-          PPSCI_LAUNCH(kf, grid_e, dim3(NTHREADS), smem_f, st, g);
-          P->launches++;
+          launch(CLS_FWD, kf, dim3(ptiles, (unsigned)((g.Nout + TN - 1) / TN)), dim3(NTHREADS), smem_f, g);
         }
       }
       if (gated && l < L && !(emb && l == 1)) post_fwd(l);
@@ -871,12 +824,9 @@ static int run(ppsci_plan* P, const CallArgs& a) {
     // ---------------- residual program + loss + output adjoints ----------------
     if (a.jets_out) {
       const long long tot = (long long)C * nc * n_out;
-      auto kc = k_copy_jets<T>;
-      ProfScope ps_(P, CLS_MISC, st);
-      PPSCI_LAUNCH(kc, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st,
-                   reinterpret_cast<const T*>(ws + cv.y), P->ld[L], (long long)nc_max * P->ld[L],
-                   reinterpret_cast<T*>(a.jets_out), (long long)a.n_points, (long long)c0, (long long)nc, C, n_out);
-      P->launches++;
+      launch(CLS_MISC, k_copy_jets<T>, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0,
+             reinterpret_cast<const T*>(ws + cv.y), P->ld[L], (long long)nc_max * P->ld[L],
+             reinterpret_cast<T*>(a.jets_out), (long long)a.n_points, (long long)c0, (long long)nc, C, n_out);
     }
     if (s.n_res > 0 && (a.want_loss || a.residual_out) && !a.ybar_in) {
       HeadArgs<T> h;
@@ -921,152 +871,108 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         h.residual_out[k] = a.residual_out ? a.residual_out[k] : nullptr;
       }
       h.loss_acc = a.want_loss ? loss_acc : nullptr;
-      auto kh = k_head<T>;
-      ProfScope ps_(P, CLS_HEAD, st);
-      PPSCI_LAUNCH(kh, dim3((unsigned)((nc + HEAD_THREADS - 1) / HEAD_THREADS)), dim3(HEAD_THREADS), 0, st, h);
-      P->launches++;
+      launch(CLS_HEAD, k_head<T>, dim3((unsigned)((nc + HEAD_THREADS - 1) / HEAD_THREADS)), dim3(HEAD_THREADS), 0, h);
     }
     if (!do_bwd || a.phase == 1) continue;
     if (a.ybar_in && a.ybar_in != static_cast<const void*>(ws + cv.ybar)) {  // output adjoints from the caller (not already in place)
       const long long tot = (long long)nc * P->ld[L];
-      auto ks = k_seed_ybar<T>;
-      ProfScope ps_(P, CLS_MISC, st);
-      PPSCI_LAUNCH(ks, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st, reinterpret_cast<const T*>(a.ybar_in),
-                   (long long)c0, (long long)nc, n_out, C, reinterpret_cast<T*>(ws + cv.ybar), P->ld[L],
-                   (long long)nc_max * P->ld[L]);
-      P->launches++;
+      launch(CLS_MISC, k_seed_ybar<T>, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, reinterpret_cast<const T*>(a.ybar_in),
+             (long long)c0, (long long)nc, n_out, C, reinterpret_cast<T*>(ws + cv.ybar), P->ld[L], (long long)nc_max * P->ld[L]);
     }
     // ---------------- adjoint ----------------
-    const T* zbar_cur = reinterpret_cast<const T*>(ws + cv.ybar);
-    int zbar_ld = P->ld[L];
-    int flip = 0;
-    // destination of Zbar_{lower}: the two ping-pong buffers
-    auto zbar_dst = [&](int) -> T* { return reinterpret_cast<T*>(ws + (flip ? cv.zbar1 : cv.zbar0)); };
     for (int l = L; l >= 1; --l) {
-      if (l == L && thin_last) {  // dW_L, db_L and Zbar_{L-1} in one streaming pass
+      if (l == L && P->thin_last) {  // dW_L, db_L and Zbar_{L-1} in one streaming pass
         LastArgs<T> f;
         memset(&f, 0, sizeof(f));
-        fill_act<T>(P, reinterpret_cast<const T*>(ws + cv.z[L - 1]), P->ld[L - 1], nc_max, A_ACT, &f.A, L - 1);
+        f.A = operand(L, c0);
         f.J = P->J;
         f.W = params + P->w_off[L];
         f.K = s.widths[L - 1];
         f.m = s.widths[L];
-        f.Ybar = zbar_cur;
+        f.Ybar = zbar(L);
         f.ldy = P->ld[L];
         f.yplane = (long long)nc_max * P->ld[L];
-        T* outp = zbar_dst(L - 1);
-        f.ZbarOut = outp;
+        f.ZbarOut = zbar(L - 1);
         f.ldo = P->ld[L - 1];
         f.oplane = (long long)nc_max * P->ld[L - 1];
         f.dW = grads + P->w_off[L];
         f.db = grads + P->b_off[L];
         f.Np = nc;
         f.pts_per_block = 64;
-        bool last_done = false;
+        void (*k)(LastArgs<T>) = k_last_bwd<T, KMAX>;
         if constexpr (sizeof(T) == 4) {
-          if (thin_vec && f.K % 4 == 0 && f.m <= 4) {
+          if (P->thin_vec && f.K % 4 == 0 && f.m <= 4) {
             f.pts_per_block = 128;
-            void (*kv)(LastArgs<float>) = nullptr;
-            PPSCI_THIN_PICK_LM(k_last_bwd_v, thin_lay, f.m, kv);
-            ProfScope ps_(P, CLS_THIN_DX, st);
-            PPSCI_LAUNCH(kv, dim3((unsigned)((f.K + 255) / 256), (unsigned)((nc + 127) / 128)), dim3(256), 0, st, f);
-            P->launches++;
-            last_done = true;
+            PPSCI_THIN_PICK_LM(k_last_bwd_v, P->thin_lay, f.m, k);
           }
         }
-        if (!last_done) {
-          auto k3 = k_last_bwd<T, KMAX>;
-          ProfScope ps_(P, CLS_THIN_DX, st);
-          PPSCI_LAUNCH(k3, dim3((unsigned)((f.K + 255) / 256), (unsigned)((nc + 63) / 64)), dim3(256), 0, st, f);
-          P->launches++;
-        }
-        zbar_cur = outp;
-        zbar_ld = P->ld[L - 1];
-        flip ^= 1;
+        const dim3 grid((unsigned)((f.K + 255) / 256), (unsigned)((nc + f.pts_per_block - 1) / f.pts_per_block));
+        launch(CLS_THIN_DX, k, grid, dim3(256), 0, f);
         continue;
       }
-      if (l == 1 && thin_first) {
+      if (l == 1 && P->thin_first) {
         FirstArgs<T> f;
         memset(&f, 0, sizeof(f));
-        fill_seed<T>(P, a.x_cols, c0, &f.A);
+        f.A = operand(1, c0);
         f.J = P->J;
         f.nf = s.widths[0];
         f.N = s.widths[1];
-        f.Zbar = zbar_cur;
-        f.ldzb = zbar_ld;
-        f.zbplane = (long long)nc_max * zbar_ld;
+        f.Zbar = zbar(1);
+        f.ldzb = P->ld[1];
+        f.zbplane = (long long)nc_max * P->ld[1];
         f.dW = grads + P->w_off[1];
         f.db = grads + P->b_off[1];
         f.Np = nc;
         f.pts_per_block = 32;
+        void (*k)(FirstArgs<T>) = k_first_dw<T, KMAX>;
         if constexpr (sizeof(T) == 4) {
-          if (thin_vec && f.N % 4 == 0) {
+          if (P->thin_vec && f.N % 4 == 0) {
             f.pts_per_block = 256;
-            void (*kv)(FirstArgs<float>) = nullptr;
-            PPSCI_THIN_PICK_L(k_first_dw_v, thin_lay, KMAX, kv);
-            ProfScope ps_(P, CLS_THIN_DW, st);
-            PPSCI_LAUNCH(kv, dim3((unsigned)((f.N + 255) / 256), (unsigned)((nc + 255) / 256)), dim3(256), 0, st, f);
-            P->launches++;
-            break;
+            PPSCI_THIN_PICK_L(k_first_dw_v, P->thin_lay, KMAX, k);
           }
         }
-        auto k4 = k_first_dw<T, KMAX>;
-        ProfScope ps_(P, CLS_THIN_DW, st);
-        PPSCI_LAUNCH(k4, dim3((unsigned)((f.N + 255) / 256), (unsigned)((nc + 31) / 32)), dim3(256), 0, st, f);
-        P->launches++;
+        const dim3 grid((unsigned)((f.N + 255) / 256), (unsigned)((nc + f.pts_per_block - 1) / f.pts_per_block));
+        launch(CLS_THIN_DW, k, grid, dim3(256), 0, f);
         break;
       }
 #ifndef PPSCI_EMUL
-      if (sizeof(T) == 4 && wg_dw_layer(P, l)) {  // dW_l and db_l on the tensor cores
-        wg::WgDwArgs w;
-        memset(&w, 0, sizeof(w));
-        if (l == 1) {  // dense first layer: the caller's matrix is the operand
-          fill_act<float>(P, reinterpret_cast<const float*>(a.x_cols[0]) + c0 * s.widths[0], s.widths[0], nc_max, A_ACT, &w.A);
-          w.A.act = PPSCI_ACT_IDENTITY;
-        } else {
-          fill_act<float>(P, reinterpret_cast<const float*>(ws + cv.z[l - 1]), P->ld[l - 1], nc_max, A_ACT, &w.A, l - 1);
+      if (P->wg_dw[l]) {  // dW_l and db_l on the tensor cores
+        if constexpr (sizeof(T) == 4) {
+          wg::WgDwArgs w;
+          memset(&w, 0, sizeof(w));
+          w.A = operand(l, c0);
+          if (l == 1) w.A.act = PPSCI_ACT_IDENTITY;  // dense first layer: the caller's matrix is the operand
+          w.J = P->J;
+          w.Zbar = zbar(l);
+          w.ldzb = P->ld[l];
+          w.zbplane = (long long)nc_max * P->ld[l];
+          w.Kdim = s.widths[l - 1];
+          w.Nout = s.widths[l];
+          w.dW = grads + P->w_off[l];
+          w.db = grads + P->b_off[l];
+          w.Np = nc;
+          // column blocks of equal width (in units of 32) up to dw_maxq(C); fan-in blocks x column blocks fastest on the
+          // grid, so the CTAs that read the same points run together and share them through L2
+          const int nq = w.Nout / 32, ncb = (nq + wg::dw_maxq(C) - 1) / wg::dw_maxq(C), bnq = (nq + ncb - 1) / ncb;
+          w.col_blocks = ncb;
+          const unsigned tiles = (unsigned)((w.Kdim + wg::DW_TK - 1) / wg::DW_TK * ncb);
+          const DwSplit sp = dw_split(P->num_sms / tiles, (nc + wg::dw_pch(C) - 1) / wg::dw_pch(C));
+          w.chunks_per_split = sp.chunks_per_split;
+          const int smem = wg::dw_smem_bytes(C, bnq);
+          const auto k = wg_dw_kernel(wg_layout(P->J), bnq);
+          CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+          launch(CLS_DW, k, dim3(tiles, sp.splits), dim3(wg::THREADS), smem, w);
         }
-        w.J = P->J;
-        w.Zbar = reinterpret_cast<const float*>(zbar_cur);
-        w.ldzb = zbar_ld;
-        w.zbplane = (long long)nc_max * zbar_ld;
-        w.Kdim = s.widths[l - 1];
-        w.Nout = s.widths[l];
-        w.dW = reinterpret_cast<float*>(grads) + P->w_off[l];
-        w.db = reinterpret_cast<float*>(grads) + P->b_off[l];
-        w.Np = nc;
-        // column blocks of equal width (in units of 32) up to dw_maxq(C); fan-in blocks x column blocks fastest on the
-        // grid, so the CTAs that read the same points run together and share them through L2
-        const int nq = w.Nout / 32, ncb = (nq + wg::dw_maxq(C) - 1) / wg::dw_maxq(C), bnq = (nq + ncb - 1) / ncb;
-        w.col_blocks = ncb;
-        const long long total_chunks = (nc + wg::dw_pch(C) - 1) / wg::dw_pch(C);
-        const unsigned tiles = (unsigned)((w.Kdim + wg::DW_TK - 1) / wg::DW_TK * ncb);
-        long long want = P->num_sms / tiles;
-        if (want < 1) want = 1;
-        if (want > total_chunks) want = total_chunks;
-        const long long cps = (total_chunks + want - 1) / want;
-        w.chunks_per_split = (int)cps;
-        const unsigned splits = (unsigned)((total_chunks + cps - 1) / cps);
-        const int smem = wg::dw_smem_bytes(C, bnq);
-        ProfScope ps_(P, CLS_DW, st);
-        PPSCI_WG_DW_LAUNCH(wg_layout(P->J), bnq, dim3(tiles, splits), smem, st, w,
-                           return fail(std::string("cudaFuncSetAttribute(k_wg_dw): ") + cudaGetErrorString(e_)));
-        P->launches++;
       } else
 #endif
       {  // dW_l, db_l
         DwArgs<T> g;
         memset(&g, 0, sizeof(g));
-        if (l == 1) fill_first<T>(P, a.x_cols, c0, nc_max, &g.A);
-        else if (gated) fill_act<T>(P, reinterpret_cast<const T*>(ws + cv.gt[l - 1]), P->ld[l - 1], nc_max, A_PLAIN, &g.A);
-        else {
-          fill_act<T>(P, reinterpret_cast<const T*>(ws + cv.z[l - 1]), P->ld[l - 1], nc_max, A_ACT, &g.A, l - 1);
-          set_actp(&g.A, l - 1);
-        }
+        g.A = operand(l, c0);
         g.J = P->J;
-        g.Zbar = zbar_cur;
-        g.ldzb = zbar_ld;
-        g.zbplane = (long long)nc_max * zbar_ld;
+        g.Zbar = zbar(l);
+        g.ldzb = P->ld[l];
+        g.zbplane = (long long)nc_max * P->ld[l];
         g.Kdim = s.widths[l - 1];
         g.Nout = s.widths[l];
         g.dW = grads + P->w_off[l];
@@ -1074,85 +980,53 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         g.Np = nc;
         g.PT = PT;
         const unsigned kt = (unsigned)((g.Kdim + TM - 1) / TM), nt = (unsigned)((g.Nout + TN - 1) / TN);
-        const long long total_chunks = (nc + PT - 1) / PT;
-        long long want = (4LL * P->num_sms + kt * nt - 1) / (kt * nt);
-        if (want < 1) want = 1;
-        if (want > total_chunks) want = total_chunks;
-        const long long cps = (total_chunks + want - 1) / want;
-        const unsigned splits = (unsigned)((total_chunks + cps - 1) / cps);
-        g.chunks_per_split = (int)cps;
-        {
-          ProfScope ps_(P, CLS_DW, st);
-          PPSCI_LAUNCH(kw, dim3(kt, nt, splits), dim3(NTHREADS), smem_w, st, g);
-          P->launches++;
-        }
+        const DwSplit sp = dw_split((4LL * P->num_sms + kt * nt - 1) / (kt * nt), (nc + PT - 1) / PT);
+        g.chunks_per_split = sp.chunks_per_split;
+        launch(CLS_DW, kw, dim3(kt, nt, sp.splits), dim3(NTHREADS), smem_w, g);
         if (gated && l == 1) {  // dWu, dbu, dWv, dbv from the adjoints the gates accumulated
-          unsigned kt_e = kt, nt_e = nt;
-          if (emb) {
-            fill_act<T>(P, reinterpret_cast<const T*>(ws + cv.gt[1]), P->ld[1], nc_max, A_PLAIN, &g.A);
-            g.Kdim = s.widths[1];
-            g.Nout = s.widths[2];
-            kt_e = (unsigned)((g.Kdim + TM - 1) / TM);
-            nt_e = (unsigned)((g.Nout + TN - 1) / TN);
-          }
+          g.A = operand(emb + 1, c0);
+          g.Kdim = s.widths[emb];
+          g.Nout = s.widths[emb + 1];
+          const dim3 grid_e((unsigned)((g.Kdim + TM - 1) / TM), (unsigned)((g.Nout + TN - 1) / TN), sp.splits);
           for (int e = 0; e < 2; ++e) {
             g.Zbar = reinterpret_cast<const T*>(ws + (e == 0 ? cv.zub : cv.zvb));
             g.ldzb = P->ld[emb + 1];
             g.zbplane = (long long)nc_max * P->ld[emb + 1];
             g.dW = grads + P->gate_w_off[e];
             g.db = grads + P->gate_b_off[e];
-            ProfScope ps_(P, CLS_DW, st);
-            PPSCI_LAUNCH(kw, dim3(kt_e, nt_e, splits), dim3(NTHREADS), smem_w, st, g);
-            P->launches++;
+            launch(CLS_DW, kw, grid_e, dim3(NTHREADS), smem_w, g);
           }
         }
       }
       if (l == 1) break;
 #ifndef PPSCI_EMUL
-      if (sizeof(T) == 4 && wg_dx_layer(P, l)) {  // Zbar_{l-1} on the tensor cores
-        wg::WgArgs w;
-        memset(&w, 0, sizeof(w));
-        fill_act<float>(P, reinterpret_cast<const float*>(zbar_cur), zbar_ld, nc_max, A_PLAIN, &w.A);
-        w.J = P->J;
-        w.Wimg = reinterpret_cast<const float*>(ws + cv.wimg + wg_imgT_offset(P, l));
-        w.Kdim = s.widths[l];
-        w.Nout = s.widths[l - 1];
-        float* outp = reinterpret_cast<float*>(zbar_dst(l - 1));
-        w.Out = outp;
-        w.ldo = P->ld[l - 1];
-        w.oplane = (long long)nc_max * P->ld[l - 1];
-        w.Np = nc;
-        const unsigned wtiles = (unsigned)((nc + wg::tile_points(C) - 1) / wg::tile_points(C));
-        w.num_tiles = (int)wtiles;
-        w.Zprev = reinterpret_cast<const float*>(ws + cv.z[l - 1]);
-        w.ldz = P->ld[l - 1];
-        w.zplane = (long long)nc_max * P->ld[l - 1];
-        w.act = act_of_layer(s, l - 1);
-        const int smem = wg::fwd_smem_bytes(w.Nout);
-        const unsigned gridx = wtiles < (unsigned)P->num_sms ? wtiles : (unsigned)P->num_sms;
-        {
-          ProfScope ps_(P, CLS_DX, st);
-          PPSCI_WG_LAUNCH(true, wg_layout(P->J), w.Nout, dim3(gridx), smem, st, w,
-                          return fail(std::string("cudaFuncSetAttribute(k_wg_layer dx): ") + cudaGetErrorString(e_)));
-          P->launches++;
+      if (P->wg_dx[l]) {  // Zbar_{l-1} on the tensor cores
+        if constexpr (sizeof(T) == 4) {
+          wg::WgArgs w;
+          memset(&w, 0, sizeof(w));
+          fill_act<T>(P, zbar(l), P->ld[l], nc_max, A_PLAIN, &w.A);
+          w.Kdim = s.widths[l];
+          w.Nout = s.widths[l - 1];
+          w.Zprev = reinterpret_cast<const T*>(ws + cv.z[l - 1]);
+          w.ldz = P->ld[l - 1];
+          w.zplane = (long long)nc_max * P->ld[l - 1];
+          w.act = act_of_layer(s, l - 1);
+          if (launch_wg(CLS_DX, true, w, P->imgT_off[l], l - 1, zbar(l - 1), nc)) return 1;
         }
-        zbar_cur = reinterpret_cast<const T*>(outp);
-        zbar_ld = P->ld[l - 1];
-        flip ^= 1;
         continue;
       }
 #endif
       {  // Zbar_{l-1}
         GemmArgs<T> g;
         memset(&g, 0, sizeof(g));
-        fill_act<T>(P, zbar_cur, zbar_ld, nc_max, A_PLAIN, &g.A);
+        fill_act<T>(P, zbar(l), P->ld[l], nc_max, A_PLAIN, &g.A);
         g.J = P->J;
         g.B = reinterpret_cast<const T*>(ws + cv.wt[l]);  // [N_l][K_l]
         g.Kdim = s.widths[l];
         g.Nout = s.widths[l - 1];
         g.ldb = s.widths[l - 1];
         g.bias = nullptr;
-        T* outp = zbar_dst(l - 1);
+        T* outp = zbar(l - 1);
         g.Out = outp;
         g.ldo = P->ld[l - 1];
         g.oplane = (long long)nc_max * P->ld[l - 1];
@@ -1167,25 +1041,18 @@ static int run(ppsci_plan* P, const CallArgs& a) {
           g.act_param_grad = grads + P->actp_off[l - 1];
           g.act_pstride = P->actp_stride;
         }
-        dim3 grid(ptiles, (unsigned)((g.Nout + TN - 1) / TN));
-        {
-          ProfScope ps_(P, CLS_DX, st);
-          PPSCI_LAUNCH(kx, grid, dim3(NTHREADS), smem_x, st, g);
-          P->launches++;
-        }
+        const dim3 grid(ptiles, (unsigned)((g.Nout + TN - 1) / TN));
+        launch(CLS_DX, kx, grid, dim3(NTHREADS), smem_x, g);
         if (gated && emb && l == 2) {  // layer 1's output also feeds the embeddings: += Zubar Wu^T + Zvbar Wv^T
           for (int e = 0; e < 2; ++e) {
             fill_act<T>(P, reinterpret_cast<const T*>(ws + (e == 0 ? cv.zub : cv.zvb)), P->ld[2], nc_max, A_PLAIN, &g.A);
             g.B = reinterpret_cast<const T*>(ws + (e == 0 ? cv.wtu : cv.wtv));
             g.accum = 1;
-            ProfScope ps_(P, CLS_DX, st);
-            PPSCI_LAUNCH(kx, grid, dim3(NTHREADS), smem_x, st, g);
-            P->launches++;
+            launch(CLS_DX, kx, grid, dim3(NTHREADS), smem_x, g);
           }
         }
         if (gated) {  // adjoint of what follows layer l-1, in place: operand adjoint -> Zbar_{l-1}
           const long long tot = (long long)nc * s.widths[l - 1];
-          ProfScope ps_(P, CLS_MISC, st);
           if (post_kind(l - 1) == 0) {  // gate; the adjoints of the embeddings' pre-activations accumulate
             GateArgs<T> ga;
             fill_gate(l - 1, nc, &ga);
@@ -1193,7 +1060,7 @@ static int run(ppsci_plan* P, const CallArgs& a) {
             ga.Zub = reinterpret_cast<T*>(ws + cv.zub);
             ga.Zvb = reinterpret_cast<T*>(ws + cv.zvb);
             ga.first = (l - 1 == (pirate ? L - 2 : L - 1)) ? 1 : 0;
-            PPSCI_LAUNCH(kgb, dim3((unsigned)((tot + 127) / 128)), dim3(128), 0, st, ga);
+            launch(CLS_MISC, k_gate_bwd<T, KMAX>, dim3((unsigned)((tot + 127) / 128)), dim3(128), 0, ga);
           } else {  // adaptive residual of a block (dLoss/dalpha reduced here), or the embedding layer's activation
             MixArgs<T> ma;
             fill_mix(l - 1, nc, &ma);
@@ -1207,22 +1074,14 @@ static int run(ppsci_plan* P, const CallArgs& a) {
               ma.use_res = pirate ? 1 : 0;  // block 0's residual path
             }
             const long long want = (tot + 127) / 128, cap = 8LL * P->num_sms;
-            PPSCI_LAUNCH(kmb, dim3((unsigned)(want < cap ? want : cap)), dim3(128), 0, st, ma);
+            launch(CLS_MISC, k_mix_bwd<T, KMAX>, dim3((unsigned)(want < cap ? want : cap)), dim3(128), 0, ma);
           }
-          P->launches++;
         }
-        zbar_cur = outp;
-        zbar_ld = P->ld[l - 1];
-        flip ^= 1;
       }
     }
   }
-  if (a.want_loss && a.loss_out && s.n_res > 0) {
-    auto kfin = k_finalize_loss<T>;
-    ProfScope ps_(P, CLS_MISC, st);
-    PPSCI_LAUNCH(kfin, dim3(1), dim3(32), 0, st, loss_acc, reinterpret_cast<T*>(a.loss_out), s.n_res);
-    P->launches++;
-  }
+  if (a.want_loss && a.loss_out && s.n_res > 0)
+    launch(CLS_MISC, k_finalize_loss<T>, dim3(1), dim3(32), 0, loss_acc, reinterpret_cast<T*>(a.loss_out), s.n_res);
   CK(cudaGetLastError());
   return 0;
 }

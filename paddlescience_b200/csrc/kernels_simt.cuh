@@ -24,9 +24,6 @@
 #define PPSCI_DYN_SMEM(name) extern __shared__ __align__(16) unsigned char name[]
 #define PPSCI_LAUNCH(kernel, grid, block, smem, stream, ...) \
   kernel<<<(grid), (block), (smem), (cudaStream_t)(stream)>>>(__VA_ARGS__)
-// one-argument kernels; `cluster` documents the __cluster_dims__ of the kernel (the emulation build needs it)
-#define PPSCI_KLAUNCH(kfn, grid, block, smem, stream, cluster, args) \
-  kfn<<<(grid), (block), (smem), (cudaStream_t)(stream)>>>(args)
 #endif
 
 namespace ppsci {

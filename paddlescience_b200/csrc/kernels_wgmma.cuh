@@ -753,27 +753,27 @@ inline bool wg_dw_ok(const ppsci_plan_spec& s, int l, const JetLayout& J) {
   return K % 4 == 0 && N % 32 == 0 && N >= 32 && N <= 256;
 }
 
-// column block of q x 32 columns (q <= dw_maxq(C)); layouts with more channels instantiate only the narrower blocks
+namespace wg {
+using Lay4444 = SLay<4, 4, 4, 4>;
+}
+// k_wg_dw instance for jet layout `lay` (wg_layout) and a column block of q x 32 columns (q <= dw_maxq(C)); layouts with
+// more channels instantiate only the narrower blocks
 #define PPSCI_WG_DW_PICK_(LAY, q)                                                                                \
   ((q) == 4   ? wg::k_wg_dw<LAY, wg::dw_q(LAY::CS, 4)>                                                          \
    : (q) == 3 ? wg::k_wg_dw<LAY, wg::dw_q(LAY::CS, 3)>                                                          \
    : (q) == 2 ? wg::k_wg_dw<LAY, 2>                                                                             \
               : wg::k_wg_dw<LAY, 1>)
-#define PPSCI_WG_DW_LAUNCH(lay, q, grid, smem, stream, args, err_expr)                                            \
-  do {                                                                                                           \
-    void (*kfn_)(decltype(args)) = nullptr;                                                                      \
-    switch (lay) {                                                                                               \
-      case LAY_22: kfn_ = PPSCI_WG_DW_PICK_(thin::Lay22, q); break;                                              \
-      case LAY_12: kfn_ = PPSCI_WG_DW_PICK_(thin::Lay12, q); break;                                              \
-      case LAY_222: kfn_ = PPSCI_WG_DW_PICK_(thin::Lay222, q); break;                                            \
-      case WG_LAY_4444: kfn_ = PPSCI_WG_DW_PICK_(wg::Lay4444, q); break;                                         \
-      default: kfn_ = PPSCI_WG_DW_PICK_(thin::LayV, q);                                                          \
-    }                                                                                                            \
-    cudaError_t e_ = cudaFuncSetAttribute(kfn_, cudaFuncAttributeMaxDynamicSharedMemorySize, (smem));            \
-    if (e_ != cudaSuccess) { err_expr; }                                                                         \
-    PPSCI_KLAUNCH(kfn_, (grid), dim3(wg::THREADS), (smem), (stream), 1, args);                                    \
-  } while (0)
+inline auto wg_dw_kernel(int lay, int q) -> void (*)(wg::WgDwArgs) {
+  switch (lay) {
+    case LAY_22: return PPSCI_WG_DW_PICK_(thin::Lay22, q);
+    case LAY_12: return PPSCI_WG_DW_PICK_(thin::Lay12, q);
+    case LAY_222: return PPSCI_WG_DW_PICK_(thin::Lay222, q);
+    case WG_LAY_4444: return PPSCI_WG_DW_PICK_(wg::Lay4444, q);
+    default: return PPSCI_WG_DW_PICK_(thin::LayV, q);
+  }
+}
 
+// k_wg_layer instance (DX: the dx variant) for jet layout `lay` and n output columns
 #define PPSCI_WG_PICK_(DX, LAY, n)                                                                               \
   ((n) == 256   ? wg::k_wg_layer<LAY, 8, DX>                                                                    \
    : (n) == 224 ? wg::k_wg_layer<LAY, 7, DX>                                                                    \
@@ -783,23 +783,16 @@ inline bool wg_dw_ok(const ppsci_plan_spec& s, int l, const JetLayout& J) {
    : (n) == 96  ? wg::k_wg_layer<LAY, 3, DX>                                                                    \
    : (n) == 64  ? wg::k_wg_layer<LAY, 2, DX>                                                                    \
                 : wg::k_wg_layer<LAY, 1, DX>)
-namespace wg {
-using Lay4444 = SLay<4, 4, 4, 4>;
+template <bool DX>
+inline auto wg_layer_kernel(int lay, int n) -> void (*)(wg::WgArgs) {
+  switch (lay) {
+    case LAY_22: return PPSCI_WG_PICK_(DX, thin::Lay22, n);
+    case LAY_12: return PPSCI_WG_PICK_(DX, thin::Lay12, n);
+    case LAY_222: return PPSCI_WG_PICK_(DX, thin::Lay222, n);
+    case WG_LAY_4444: return PPSCI_WG_PICK_(DX, wg::Lay4444, n);
+    default: return PPSCI_WG_PICK_(DX, thin::LayV, n);
+  }
 }
-#define PPSCI_WG_LAUNCH(DX, lay, n, grid, smem, stream, args, err_expr)                                           \
-  do {                                                                                                           \
-    void (*kfn_)(decltype(args)) = nullptr;                                                                      \
-    switch (lay) {                                                                                               \
-      case LAY_22: kfn_ = PPSCI_WG_PICK_(DX, thin::Lay22, n); break;                                             \
-      case LAY_12: kfn_ = PPSCI_WG_PICK_(DX, thin::Lay12, n); break;                                             \
-      case LAY_222: kfn_ = PPSCI_WG_PICK_(DX, thin::Lay222, n); break;                                           \
-      case WG_LAY_4444: kfn_ = PPSCI_WG_PICK_(DX, wg::Lay4444, n); break;                                        \
-      default: kfn_ = PPSCI_WG_PICK_(DX, thin::LayV, n);                                                         \
-    }                                                                                                            \
-    cudaError_t e_ = cudaFuncSetAttribute(kfn_, cudaFuncAttributeMaxDynamicSharedMemorySize, (smem));            \
-    if (e_ != cudaSuccess) { err_expr; }                                                                         \
-    PPSCI_KLAUNCH(kfn_, (grid), dim3(wg::THREADS), (smem), (stream), 1, args);                                    \
-  } while (0)
 
 }  // namespace ppsci
 #endif  // PPSCI_EMUL

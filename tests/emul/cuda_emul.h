@@ -245,8 +245,6 @@ inline unsigned char* dyn_smem() { return t_cta->smem; }
 #define PPSCI_DYN_SMEM(name) unsigned char* name = emul::dyn_smem()
 #define PPSCI_LAUNCH(kernel, grid, block, smem, stream, ...) \
   emul::launch((grid), (block), (smem), [&]() { kernel(__VA_ARGS__); })
-#define PPSCI_KLAUNCH(kfn, grid, block, smem, stream, cluster, args) \
-  emul::launch((grid), (block), (smem), [&]() { kfn(args); }, (cluster))
 
 struct __attribute__((aligned(16))) float4 { float x, y, z, w; };
 struct __attribute__((aligned(16))) double2 { double x, y; };
