@@ -45,51 +45,18 @@ __device__ __forceinline__ void gate_act_jet(int act, const JetLayout& J, const 
   zj[0] = z[0];
   act_coef<T, KMAX + 1>(act, zj[0], y0, s);
   y[0] = y0;
-  for (int d = 0; d < J.n_dir; ++d) {
-    const int K = J.dir_order[d];
-    const int base = J.dir_base[d];
-    T zz[4], yy[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      zz[q] = (q < KMAX && q < K) ? z[(long long)(base + q) * plane] : T(0);
-      yy[q] = T(0);
-    }
-    jet_fwd_dir<T, KMAX>(s, zz, yy);
-#pragma unroll
-    for (int q = 0; q < KMAX; ++q)
-      if (q < K) {
-        zj[base + q] = zz[q];
-        y[base + q] = yy[q];
-      }
-  }
+  jet_fwd<T, DynLay<KMAX>>(J, s, [&](int c) { return zj[c] = z[(long long)c * plane]; }, [&](int c, T v) { y[c] = v; });
 }
 
 // adjoint of y = act(z): yb -> zb, stored (accumulate = false) or added (true) at out[c * plane]
 template <typename T, int KMAX>
 __device__ __forceinline__ void gate_act_adj(const JetLayout& J, const T (&s)[6], const T (&zj)[GATE_MAXC],
                                              const T (&yb)[GATE_MAXC], T* out, long long plane, bool accumulate) {
-  T sb[5] = {T(0), T(0), T(0), T(0), T(0)};
-  for (int d = 0; d < J.n_dir; ++d) {
-    const int K = J.dir_order[d];
-    const int base = J.dir_base[d];
-    T zz[4], y4[4], zb[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const bool on = (q < KMAX && q < K);
-      zz[q] = on ? zj[base + q] : T(0);
-      y4[q] = on ? yb[base + q] : T(0);
-      zb[q] = T(0);
-    }
-    jet_adj_dir<T, KMAX>(s, zz, y4, zb, sb);
-#pragma unroll
-    for (int q = 0; q < KMAX; ++q)
-      if (q < K) {
-        T* o = out + (long long)(base + q) * plane;
-        *o = accumulate ? *o + zb[q] : zb[q];
-      }
-  }
-  const T z0b = jet_adj_z0<T, KMAX>(s, yb[0], sb);
-  out[0] = accumulate ? out[0] + z0b : z0b;
+  auto put = [&](int c, T v) {
+    T* o = out + (long long)c * plane;
+    *o = accumulate ? *o + v : v;
+  };
+  put(0, jet_adj<T, DynLay<KMAX>>(J, s, [&](int c) { return zj[c]; }, [&](int c) { return yb[c]; }, put));
 }
 
 template <typename T, int KMAX>

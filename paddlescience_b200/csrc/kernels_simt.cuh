@@ -16,8 +16,7 @@
 //                  MSELoss.forward (ppsci/loss/mse.py:82-106), mtl.Sum (loss/mtl/sum.py:45-60)
 #pragma once
 
-#include "jet_math.h"
-#include "ppsci_b200.h"
+#include "jet_layout.cuh"
 
 #ifndef PPSCI_EMUL
 #include <cuda_runtime.h>
@@ -33,13 +32,6 @@ constexpr int TMS = TM + 4;  // padded smem row stride of the k-major A tile
 constexpr int KC = 16;       // reduction chunk of the fwd / dx GEMMs
 constexpr int RC = 32;       // reduction (row) chunk of the dW GEMM
 constexpr int NTHREADS = 256;
-
-struct JetLayout {
-  int C;
-  int n_dir;
-  int dir_order[PPSCI_MAX_DIR];
-  int dir_base[PPSCI_MAX_DIR];  // channel index of order-1 coefficient of direction d
-};
 
 struct SeedSpec {
   int n_in;
@@ -87,17 +79,7 @@ __device__ __forceinline__ void produce_a(const AOperand<T>& A, const JetLayout&
     if (A.act_param) act_coef_p<T, KMAX>(A.act, z[0], A.act_param[(long long)k * A.act_pstride], y0, s);
     else act_coef<T, KMAX>(A.act, z[0], y0, s);
     st(0, y0);
-    for (int d = 0; d < J.n_dir; ++d) {
-      const int K = J.dir_order[d];
-      const int base = J.dir_base[d];
-      T zz[4], yy[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) zz[q] = (q < KMAX && q < K) ? z[(long long)(base + q) * A.plane] : T(0);
-      jet_fwd_dir<T, KMAX>(s, zz, yy);
-#pragma unroll
-      for (int q = 0; q < KMAX; ++q)
-        if (q < K) st(base + q, yy[q]);
-    }
+    jet_fwd<T, DynLay<KMAX>>(J, s, [&](int c) { return z[(long long)c * A.plane]; }, st);
     return;
   }
   // A_SEED: feature k of the (period-embedded) network input, Taylor-expanded along each direction
@@ -116,35 +98,6 @@ __device__ __forceinline__ void produce_a(const AOperand<T>& A, const JetLayout&
 #pragma unroll
     for (int q = 0; q < KMAX; ++q)
       if (q < K) st(base + q, co[q + 1]);
-  }
-}
-
-// Same arithmetic as produce_a's A_PLAIN / A_ACT branches, but the C channel values of the element
-// come from a caller-supplied loader ld(c) (e.g. a shared-memory staging tile).
-template <typename T, int KMAX, typename Ld, typename St>
-__device__ __forceinline__ void produce_from(int mode, int act, const JetLayout& J, bool valid, Ld ld, St st) {
-  if (!valid) {
-    for (int c = 0; c < J.C; ++c) st(c, T(0));
-    return;
-  }
-  if (mode == A_PLAIN) {
-    for (int c = 0; c < J.C; ++c) st(c, ld(c));
-    return;
-  }
-  T s[6];
-  T y0;
-  act_coef<T, KMAX>(act, ld(0), y0, s);
-  st(0, y0);
-  for (int d = 0; d < J.n_dir; ++d) {
-    const int K = J.dir_order[d];
-    const int base = J.dir_base[d];
-    T zz[4], yy[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) zz[q] = (q < KMAX && q < K) ? ld(base + q) : T(0);
-    jet_fwd_dir<T, KMAX>(s, zz, yy);
-#pragma unroll
-    for (int q = 0; q < KMAX; ++q)
-      if (q < K) st(base + q, yy[q]);
   }
 }
 
@@ -306,6 +259,8 @@ __global__ void __launch_bounds__(NTHREADS) k_gemm_dx(GemmArgs<T> g) {
     if (p >= g.Np || n >= g.Nout) continue;
     const T* z = g.Zprev + p * g.ldz + n;
     T* zb_out = g.Out + p * g.ldo + n;
+    auto ldz = [&](int c) { return z[(long long)c * g.zplane]; };
+    auto ldyb = [&](int c) { return Cs[(c * TP + pl) * TN + nn]; };
     T s[6];
     T y0;
     T qb[6];
@@ -317,35 +272,14 @@ __global__ void __launch_bounds__(NTHREADS) k_gemm_dx(GemmArgs<T> g) {
     } else {
       act_coef<T, KMAX + 1>(g.act, z[0], y0, s);
     }
-    const T y0b = Cs[pl * TN + nn];
-    if (g.act_param) bacc = y0b * qb[0];
-    T sb[5] = {T(0), T(0), T(0), T(0), T(0)};
-    for (int d = 0; d < g.J.n_dir; ++d) {
-      const int K = g.J.dir_order[d];
-      const int base = g.J.dir_base[d];
-      T zz[4], yb[4], zb[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const bool on = (q < KMAX && q < K);
-        zz[q] = on ? z[(long long)(base + q) * g.zplane] : T(0);
-        yb[q] = on ? Cs[((base + q) * TP + pl) * TN + nn] : T(0);
-        zb[q] = T(0);
-      }
-      jet_adj_dir<T, KMAX>(s, zz, yb, zb, sb);
-      if (g.act_param) {  // dLoss/dbeta += <adjoint of the activation's output jets, jets of dy/dbeta>
-        T wq[4] = {T(0), T(0), T(0), T(0)};
-        jet_fwd_dir<T, KMAX>(qb, zz, wq);
-#pragma unroll
-        for (int qq = 0; qq < KMAX; ++qq) bacc += yb[qq] * wq[qq];
-      }
-#pragma unroll
-      for (int q = 0; q < KMAX; ++q)
-        if (q < K) {
-          T* o = zb_out + (long long)(base + q) * g.oplane;
-          *o = g.accum ? *o + zb[q] : zb[q];
-        }
+    if (g.act_param) {  // dLoss/dbeta = <adjoint of the activation's output jets, jets of dy/dbeta>
+      bacc = ldyb(0) * qb[0];
+      jet_fwd<T, DynLay<KMAX>>(g.J, qb, ldz, [&](int c, T v) { bacc += ldyb(c) * v; });
     }
-    const T z0b = jet_adj_z0<T, KMAX>(s, y0b, sb);
+    const T z0b = jet_adj<T, DynLay<KMAX>>(g.J, s, ldz, ldyb, [&](int c, T v) {
+      T* o = zb_out + (long long)c * g.oplane;
+      *o = g.accum ? *o + v : v;
+    });
     zb_out[0] = g.accum ? zb_out[0] + z0b : z0b;
     bsum += bacc;
   }
@@ -599,48 +533,32 @@ __global__ void __launch_bounds__(256) k_last_bwd(LastArgs<T> g) {
       const T* yb = g.Ybar + p * g.ldy;  // + c*yplane + j   (same address for the whole block: broadcast)
       const T* z = g.A.Z + p * g.A.ld + k;
       T* zb_out = g.ZbarOut + p * g.ldo + k;
+      auto ldz = [&](int c) { return z[(long long)c * g.A.plane]; };
+      auto abar = [&](int c) {  // adjoint of activation jet channel c: sum_j Ybar[c][p][j] W[k][j]
+        const T* ybc = yb + (long long)c * g.yplane;
+        T a = T(0);
+#pragma unroll
+        for (int j = 0; j < THIN_MAXM; ++j)
+          if (j < g.m) a += ybc[j] * w[j];
+        return a;
+      };
       T s[6];
       T y0;
       act_coef<T, KMAX + 1>(g.A.act, z[0], y0, s);
-      T y0b = T(0);
 #pragma unroll
       for (int j = 0; j < THIN_MAXM; ++j)
         if (j < g.m) {
           const T ybj = yb[j];
-          y0b += ybj * w[j];
           dwacc[j] += y0 * ybj;
           if (do_db) dbacc[j] += ybj;
         }
-      T sb[5] = {T(0), T(0), T(0), T(0), T(0)};
-      for (int d = 0; d < g.J.n_dir; ++d) {
-        const int Kd = g.J.dir_order[d];
-        const int cb = g.J.dir_base[d];
-        T zz[4], yy[4], ybq[4], zbq[4];
+      jet_fwd<T, DynLay<KMAX>>(g.J, s, ldz, [&](int c, T v) {
+        const T* ybc = yb + (long long)c * g.yplane;
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          zz[q] = (q < KMAX && q < Kd) ? z[(long long)(cb + q) * g.A.plane] : T(0);
-          ybq[q] = T(0);
-          zbq[q] = T(0);
-        }
-        jet_fwd_dir<T, KMAX>(s, zz, yy);
-#pragma unroll
-        for (int q = 0; q < KMAX; ++q)
-          if (q < Kd) {
-            const T* ybc = yb + (long long)(cb + q) * g.yplane;
-#pragma unroll
-            for (int j = 0; j < THIN_MAXM; ++j)
-              if (j < g.m) {
-                const T ybj = ybc[j];
-                ybq[q] += ybj * w[j];
-                dwacc[j] += yy[q] * ybj;
-              }
-          }
-        jet_adj_dir<T, KMAX>(s, zz, ybq, zbq, sb);
-#pragma unroll
-        for (int q = 0; q < KMAX; ++q)
-          if (q < Kd) zb_out[(long long)(cb + q) * g.oplane] = zbq[q];
-      }
-      zb_out[0] = jet_adj_z0<T, KMAX>(s, y0b, sb);
+        for (int j = 0; j < THIN_MAXM; ++j)
+          if (j < g.m) dwacc[j] += v * ybc[j];
+      });
+      zb_out[0] = jet_adj<T, DynLay<KMAX>>(g.J, s, ldz, abar, [&](int c, T v) { zb_out[(long long)c * g.oplane] = v; });
     }
 #pragma unroll
     for (int j = 0; j < THIN_MAXM; ++j)

@@ -8,7 +8,7 @@
 // Same arithmetic (jet_math.h); the generic kernels remain the fallback (fp64, runtime layouts, odd widths) and
 // the on-GPU cross-check (PPSCI_B200_NO_THINV=1).
 #pragma once
-#include "jet_layout.cuh"
+#include "kernels_simt.cuh"
 
 namespace ppsci {
 namespace thin {
@@ -137,30 +137,6 @@ __global__ void __launch_bounds__(256) k_first_dw_v(FirstArgs<float> g) {
   }
 }
 
-// activation jets of 4 consecutive hidden units: a[c][t] from z[c] (float4 along k)
-template <class L, int NS>
-__device__ __forceinline__ void act_jets4(int act, const JetLayout& J, const float4 (&z)[L::CS], float (&a)[L::CS][4],
-                                          float (&sc)[4][6]) {
-  constexpr int CS = L::CS;
-#pragma unroll
-  for (int t = 0; t < 4; ++t) {
-    float y0;
-    act_coef<float, NS>(act, f4c(z[0], t), y0, sc[t]);
-    a[0][t] = y0;
-#pragma unroll
-    for (int d = 0; d < L::ND; ++d) {
-      const int K = L::order(J, d), cb = L::cbase(J, d);
-      float zz[4], yy[4];
-#pragma unroll
-      for (int o = 0; o < 4; ++o) zz[o] = (o < L::KM && o < K && cb + o < CS) ? f4c(z[(cb + o) < CS ? cb + o : 0], t) : 0.f;
-      jet_fwd_dir<float, L::KM>(sc[t], zz, yy);
-#pragma unroll
-      for (int o = 0; o < L::KM; ++o)
-        if (o < K && cb + o < CS) a[cb + o][t] = yy[o];
-    }
-  }
-}
-
 // Y[c][p][j] = sum_k act_jets(Z_{L-1})[c][p][k] W[k][j] (+ b[j] on the value channel); one warp per point,
 // lanes along k in quads.
 template <class L, int M>
@@ -179,8 +155,14 @@ __global__ void __launch_bounds__(256) k_last_fwd_v(LastArgs<float> g) {
     float4 z[CS];
 #pragma unroll
     for (int c = 0; c < CS; ++c) z[c] = __ldg(reinterpret_cast<const float4*>(zp + (long long)c * g.A.plane));
-    float a[CS][4], sc[4][6];
-    act_jets4<L, L::KM>(g.A.act, g.J, z, a, sc);
+    float a[CS][4];  // activation jets of the 4 hidden units
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      float sc[6], y0;
+      act_coef<float, L::KM>(g.A.act, f4c(z[0], t), y0, sc);
+      a[0][t] = y0;
+      jet_fwd<float, L>(g.J, sc, [&](int c) { return f4c(z[c], t); }, [&](int c, float v) { a[c][t] = v; });
+    }
 #pragma unroll
     for (int t = 0; t < 4; ++t) {
       float w[M];
@@ -241,41 +223,22 @@ __global__ void __launch_bounds__(256) k_last_bwd_v(LastArgs<float> g) {
       float ob[CS][4];
 #pragma unroll
       for (int t = 0; t < 4; ++t) {
+        auto ldz = [&](int c) { return f4c(z[c], t); };
+        auto abar = [&](int c) {  // adjoint of activation jet channel c of unit 4 kq + t
+          float a = 0.f;
+#pragma unroll
+          for (int j = 0; j < M; ++j) a += yb[c][j] * w[t][j];
+          return a;
+        };
         float sc[6], y0;
         act_coef<float, L::KM + 1>(g.A.act, f4c(z[0], t), y0, sc);
-        float y0b = 0.f;
 #pragma unroll
-        for (int j = 0; j < M; ++j) {
-          y0b += yb[0][j] * w[t][j];
-          dwacc[t][j] += y0 * yb[0][j];
-        }
-        float sb[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+        for (int j = 0; j < M; ++j) dwacc[t][j] += y0 * yb[0][j];
+        jet_fwd<float, L>(g.J, sc, ldz, [&](int c, float v) {
 #pragma unroll
-        for (int d = 0; d < L::ND; ++d) {
-          const int K = L::order(g.J, d), cb = L::cbase(g.J, d);
-          float zz[4], yy[4], ybq[4], zbq[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            zz[q] = (q < L::KM && q < K && cb + q < CS) ? f4c(z[(cb + q) < CS ? cb + q : 0], t) : 0.f;
-            ybq[q] = 0.f;
-            zbq[q] = 0.f;
-          }
-          jet_fwd_dir<float, L::KM>(sc, zz, yy);
-#pragma unroll
-          for (int q = 0; q < L::KM; ++q)
-            if (q < K && cb + q < CS) {
-#pragma unroll
-              for (int j = 0; j < M; ++j) {
-                ybq[q] += yb[cb + q][j] * w[t][j];
-                dwacc[t][j] += yy[q] * yb[cb + q][j];
-              }
-            }
-          jet_adj_dir<float, L::KM>(sc, zz, ybq, zbq, sb);
-#pragma unroll
-          for (int q = 0; q < L::KM; ++q)
-            if (q < K && cb + q < CS) ob[cb + q][t] = zbq[q];
-        }
-        ob[0][t] = jet_adj_z0<float, L::KM>(sc, y0b, sb);
+          for (int j = 0; j < M; ++j) dwacc[t][j] += v * yb[c][j];
+        });
+        ob[0][t] = jet_adj<float, L>(g.J, sc, ldz, abar, [&](int c, float v) { ob[c][t] = v; });
       }
       float* out = g.ZbarOut + p * g.ldo + 4 * kq;
 #pragma unroll

@@ -255,17 +255,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_layer(WgArgs g) {
             float y0;
             act_coef<float, L::KM>(act, comp(z[0]), y0, sc);
             yout[0][t] = valid ? y0 : 0.f;
-#pragma unroll
-            for (int d = 0; d < L::ND; ++d) {
-              const int K = L::order(g.J, d), cb = L::cbase(g.J, d);
-              float zz[4], yy[4];
-#pragma unroll
-              for (int o = 0; o < 4; ++o) zz[o] = (o < L::KM && o < K) ? comp(z[(cb + o) < CS ? (cb + o) : 0]) : 0.f;
-              jet_fwd_dir<float, L::KM>(sc, zz, yy);
-#pragma unroll
-              for (int o = 0; o < L::KM; ++o)
-                if (o < K && cb + o < CS) yout[cb + o][t] = valid ? yy[o] : 0.f;
-            }
+            jet_fwd<float, L>(g.J, sc, [&](int c) { return comp(z[c]); }, [&](int c, float v) { yout[c][t] = valid ? v : 0.f; });
           }
         }
 #pragma unroll
@@ -379,24 +369,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_layer(WgArgs g) {
           float sc[6];
           float y0;
           act_coef<float, L::KM + 1>(g.act, comp(zc[0]), y0, sc);
-          float sb[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-          for (int d = 0; d < L::ND; ++d) {
-            const int K = L::order(g.J, d), cbs = L::cbase(g.J, d);
-            float zz[4], yb[4], zbv[4];
-#pragma unroll
-            for (int o = 0; o < 4; ++o) {
-              const bool on = (o < L::KM && o < K && cbs + o < CS);
-              zz[o] = on ? comp(zc[on ? cbs + o : 0]) : 0.f;
-              yb[o] = on ? comp(xc[on ? cbs + o : 0]) : 0.f;
-              zbv[o] = 0.f;
-            }
-            jet_adj_dir<float, L::KM>(sc, zz, yb, zbv, sb);
-#pragma unroll
-            for (int o = 0; o < L::KM; ++o)
-              if (o < K && cbs + o < CS) ob[cbs + o][t] = zbv[o];
-          }
-          ob[0][t] = jet_adj_z0<float, L::KM>(sc, comp(xc[0]), sb);
+          ob[0][t] = jet_adj<float, L>(g.J, sc, [&](int c) { return comp(zc[c]); }, [&](int c) { return comp(xc[c]); },
+                                       [&](int c, float v) { ob[c][t] = v; });
         }
         float* out = g.Out + p * g.ldo + 4 * q;
 #pragma unroll
@@ -497,24 +471,6 @@ __device__ __forceinline__ void wgmma_tf32_rA_m64n32(float (&d)[16], const uint3
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
         "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1u));
-}
-
-// activation jets y[0 .. CS) of one (point, unit) from its pre-activation jets z[0 .. CS)
-template <class L>
-__device__ __forceinline__ void act_jets(int act, const JetLayout& J, const float (&z)[L::CS], float (&y)[L::CS]) {
-  float sc[6];
-  act_coef<float, L::KM>(act, z[0], y[0], sc);
-#pragma unroll
-  for (int d = 0; d < L::ND; ++d) {
-    const int K = L::order(J, d), cb = L::cbase(J, d);
-    float zz[4], yy[4];
-#pragma unroll
-    for (int o = 0; o < 4; ++o) zz[o] = (o < L::KM && o < K) ? z[(cb + o) < L::CS ? (cb + o) : 0] : 0.f;
-    jet_fwd_dir<float, L::KM>(sc, zz, yy);
-#pragma unroll
-    for (int o = 0; o < L::KM; ++o)
-      if (o < K && cb + o < L::CS) y[cb + o] = yy[o];
-  }
 }
 
 template <class L, int BNQ>
@@ -645,10 +601,11 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_dw(WgDwArgs g) {
     for (int qq = 0; qq < QPC; ++qq)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        float z[CS];
+        float z[CS], sc[6];
 #pragma unroll
         for (int c = 0; c < CS; ++c) z[c] = *za_at(qq, h, c);
-        act_jets<L>(act, g.J, z, av[qq][h]);
+        act_coef<float, L::KM>(act, z[0], av[qq][h][0], sc);
+        jet_fwd<float, L>(g.J, sc, [&](int c) { return z[c]; }, [&](int c, float v) { av[qq][h][c] = v; });
       }
     if (ch + 1 < ch_end) load_a(ch + 1);
     fence_proxy_async();
