@@ -26,6 +26,14 @@ static int fail(const std::string& msg) {
   return 1;
 }
 
+// f(T()) for the element type T of dtype (PPSCI_F32 / PPSCI_F64); any other dtype fails as "<what>: bad dtype"
+template <class F>
+static int with_dtype(int dtype, const char* what, F f) {
+  if (dtype == PPSCI_F64) return f(double());
+  if (dtype == PPSCI_F32) return f(float());
+  return fail(std::string(what) + ": bad dtype");
+}
+
 #define CK(call)                                                                              \
   do {                                                                                        \
     cudaError_t e_ = (call);                                                                  \
@@ -67,11 +75,10 @@ struct ppsci_plan {
   size_t img_off[PPSCI_MAX_LAYERS + 1] = {};
   size_t imgT_off[PPSCI_MAX_LAYERS + 1] = {};
   size_t img_bytes = 0;
-  // first / last layer on the thin kernels (kernels_thin.cuh); thin_vec: the vectorised ones, jet layout thin_lay
+  // first / last layer on the thin kernels (kernels_thin.cuh); thin_vec: the vectorised ones (a jet layout of ThinLays)
   bool thin_first = false;
   bool thin_last = false;
   bool thin_vec = false;
-  int thin_lay = 0;
   // device copies of the residual program
   int* d_prog = nullptr;
   double* d_consts = nullptr;
@@ -135,7 +142,6 @@ static inline int gate_emb(const ppsci_plan_spec& s) { return (s.gated == 2 || (
 
 // activation applied to the output of linear layer `lin` (1-based)
 static inline int act_of_layer(const ppsci_plan_spec& s, int lin) { return (lin == 1 && s.act_first >= 0) ? s.act_first : s.act; }
-static inline bool act_has_param(int act) { return act == PPSCI_ACT_STAN || act == PPSCI_ACT_SWISH_B; }
 
 static void carve(const ppsci_plan* P, int64_t nc, Carve* cv) {
   const size_t es = P->spec.dtype == PPSCI_F64 ? 8 : 4;
@@ -360,14 +366,14 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
   }
 #ifndef PPSCI_EMUL
   if (const char* m = getenv("PPSCI_B200_TC_MASK")) P->tc_mask = atoi(m);
-  for (int l = 2; l <= s->n_layers && s->backend != 1; ++l)
-    if (((P->tc_mask & 1) && wg_fwd_ok(*s, l, P->J)) || ((P->tc_mask & 2) && wg_dx_ok(*s, l, P->J)) ||
-        ((P->tc_mask & 4) && wg_dw_ok(*s, l, P->J)))
+  const bool wg_plan = s->backend != 1 && wg_plan_ok(*s, P->J);
+  for (int l = 2; l <= s->n_layers && wg_plan; ++l)
+    if (((P->tc_mask & 1) && wg_fwd_ok(*s, l)) || ((P->tc_mask & 2) && wg_dx_ok(*s, l)) || ((P->tc_mask & 4) && wg_dw_ok(*s, l)))
       P->use_wg = true;
   for (int l = 1; l <= s->n_layers && P->use_wg; ++l) {  // use_wg also gates a dense first layer
-    P->wg_fwd[l] = (P->tc_mask & 1) && wg_fwd_ok(*s, l, P->J);
-    P->wg_dx[l] = (P->tc_mask & 2) && wg_dx_ok(*s, l, P->J);
-    P->wg_dw[l] = (P->tc_mask & 4) && wg_dw_ok(*s, l, P->J);
+    P->wg_fwd[l] = (P->tc_mask & 1) && wg_fwd_ok(*s, l);
+    P->wg_dx[l] = (P->tc_mask & 2) && wg_dx_ok(*s, l);
+    P->wg_dw[l] = (P->tc_mask & 4) && wg_dw_ok(*s, l);
   }
 #endif
   for (int l = 1; l <= s->n_layers; ++l) {  // the forward images first; layer 1: contraction padded to the chunk width
@@ -381,8 +387,7 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
   const bool thin_on = getenv("PPSCI_B200_NO_THIN") == nullptr;
   P->thin_first = thin_on && s->n_layers >= 2 && s->widths[0] <= THIN_MAXF && !s->dense_in && !s->gated;
   P->thin_last = thin_on && s->n_layers >= 2 && n_out <= THIN_MAXM && C * n_out <= THIN_MAXCM && !s->gated && !act_has_param(s->act);
-  P->thin_lay = pick_layout(P->J, PPSCI_ACT_TANH);
-  P->thin_vec = s->dtype == PPSCI_F32 && P->thin_lay != LAY_DYN && getenv("PPSCI_B200_NO_THINV") == nullptr;
+  P->thin_vec = s->dtype == PPSCI_F32 && with_lay(ThinLays{}, P->J, [](auto) {}) && getenv("PPSCI_B200_NO_THINV") == nullptr;
   if (s->backend == 2 && !P->use_wg) {
     delete P;
     return fail("plan_create: backend=2 (tensor cores) requested but the plan is not eligible (needs f32, hidden widths that "
@@ -662,7 +667,12 @@ static int run(ppsci_plan* P, const CallArgs& a) {
     const unsigned tiles = (unsigned)((nc + wg::tile_points(C) - 1) / wg::tile_points(C));
     w.num_tiles = (int)tiles;
     const int smem = wg::fwd_smem_bytes(w.Nout);
-    const auto k = dx ? wg_layer_kernel<true>(wg_layout(P->J), w.Nout) : wg_layer_kernel<false>(wg_layout(P->J), w.Nout);
+    void (*k)(wg::WgArgs) = nullptr;
+    with_lay(WgLays{}, P->J, [&](auto lay) {
+      with_int<8>(w.Nout / 32, [&](auto nq) {
+        k = dx ? wg::k_wg_layer<decltype(lay), nq, true> : wg::k_wg_layer<decltype(lay), nq, false>;
+      });
+    });
     CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     launch(cls, k, dim3(tiles < (unsigned)P->num_sms ? tiles : (unsigned)P->num_sms), dim3(wg::THREADS), smem, w);
     return 0;
@@ -728,7 +738,7 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         dim3 grid((unsigned)((nc * f.N + 255) / 256));
         if constexpr (sizeof(T) == 4) {
           if (P->thin_vec && f.N % 4 == 0) {  // compile-time layout, 128-bit stores, seeds staged once per point
-            PPSCI_THIN_PICK_L(k_first_fwd_v, P->thin_lay, KMAX, k);
+            with_lay(ThinLays{}, P->J, [&](auto lay) { k = thin::k_first_fwd_v<decltype(lay)>; });
             grid = dim3((unsigned)((nc + thin::PB - 1) / thin::PB));
           }
         }
@@ -750,7 +760,8 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         f.Np = nc;
         void (*k)(LastArgs<T>) = k_last_fwd<T, KMAX>;
         if constexpr (sizeof(T) == 4) {
-          if (P->thin_vec && f.K % 4 == 0 && f.m <= 4) PPSCI_THIN_PICK_LM(k_last_fwd_v, P->thin_lay, f.m, k);
+          if (P->thin_vec && f.K % 4 == 0 && f.m <= 4)
+            with_lay(ThinLays{}, P->J, [&](auto lay) { with_int<4>(f.m, [&](auto m) { k = thin::k_last_fwd_v<decltype(lay), m>; }); });
         }
         launch(CLS_THIN_FWD, k, dim3((unsigned)((nc + 7) / 8)), dim3(256), 0, f);
         continue;
@@ -903,7 +914,7 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         if constexpr (sizeof(T) == 4) {
           if (P->thin_vec && f.K % 4 == 0 && f.m <= 4) {
             f.pts_per_block = 128;
-            PPSCI_THIN_PICK_LM(k_last_bwd_v, P->thin_lay, f.m, k);
+            with_lay(ThinLays{}, P->J, [&](auto lay) { with_int<4>(f.m, [&](auto m) { k = thin::k_last_bwd_v<decltype(lay), m>; }); });
           }
         }
         const dim3 grid((unsigned)((f.K + 255) / 256), (unsigned)((nc + f.pts_per_block - 1) / f.pts_per_block));
@@ -928,7 +939,7 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         if constexpr (sizeof(T) == 4) {
           if (P->thin_vec && f.N % 4 == 0) {
             f.pts_per_block = 256;
-            PPSCI_THIN_PICK_L(k_first_dw_v, P->thin_lay, KMAX, k);
+            with_lay(ThinLays{}, P->J, [&](auto lay) { k = thin::k_first_dw_v<decltype(lay)>; });
           }
         }
         const dim3 grid((unsigned)((f.N + 255) / 256), (unsigned)((nc + f.pts_per_block - 1) / f.pts_per_block));
@@ -959,7 +970,12 @@ static int run(ppsci_plan* P, const CallArgs& a) {
           const DwSplit sp = dw_split(P->num_sms / tiles, (nc + wg::dw_pch(C) - 1) / wg::dw_pch(C));
           w.chunks_per_split = sp.chunks_per_split;
           const int smem = wg::dw_smem_bytes(C, bnq);
-          const auto k = wg_dw_kernel(wg_layout(P->J), bnq);
+          void (*k)(wg::WgDwArgs) = nullptr;
+          with_lay(WgLays{}, P->J, [&](auto lay) {
+            with_int<4>(bnq, [&](auto q) {  // bnq <= dw_maxq(C): the wider blocks of a layout are never instantiated
+              if constexpr (q <= wg::dw_maxq(decltype(lay)::CS)) k = wg::k_wg_dw<decltype(lay), q>;
+            });
+          });
           CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
           launch(CLS_DW, k, dim3(tiles, sp.splits), dim3(wg::THREADS), smem, w);
         }
@@ -1104,8 +1120,7 @@ static int dispatch(ppsci_plan* P, const CallArgs& a) {
     for (int i = 0; i < P->spec.n_aux; ++i)
       if (!a.aux_cols[i]) return fail("null aux column " + std::to_string(i));
   }
-  if (P->spec.dtype == PPSCI_F64) return dispatch_k<double>(P, a);
-  return dispatch_k<float>(P, a);
+  return with_dtype(P->spec.dtype, "plan", [&](auto zero) { return dispatch_k<decltype(zero)>(P, a); });
 }
 
 extern "C" int ppsci_b200_plan_set_aux_grad(ppsci_plan* plan, int32_t aux_index, double* grad_dev) {
@@ -1211,21 +1226,14 @@ extern "C" int ppsci_b200_deeponet_head(int32_t dtype, int32_t act, const void* 
   if (act_has_param(act)) return fail("deeponet_head: activations with a trainable parameter are not offered here");
   const long long warps = n < 132LL * 64 ? n : 132LL * 64;  // 8 warps per block
   const unsigned blocks = (unsigned)((warps + 7) / 8);
-  if (dtype == PPSCI_F64) {
-    auto k = k_deeponet_head<double>;
-    PPSCI_LAUNCH(k, dim3(blocks), dim3(256), 0, stream, (const double*)b, (const double*)t, (const double*)bias, act,
-                 (const double*)label, (const double*)weight, (long long)n, n_features, coef, (double*)g_out, loss_acc,
-                 (double*)bbar, (double*)tbar, (double*)dbias);
-  } else if (dtype == PPSCI_F32) {
-    auto k = k_deeponet_head<float>;
-    PPSCI_LAUNCH(k, dim3(blocks), dim3(256), 0, stream, (const float*)b, (const float*)t, (const float*)bias, act,
-                 (const float*)label, (const float*)weight, (long long)n, n_features, coef, (float*)g_out, loss_acc,
-                 (float*)bbar, (float*)tbar, (float*)dbias);
-  } else {
-    return fail("deeponet_head: bad dtype");
-  }
-  CK(cudaGetLastError());
-  return 0;
+  return with_dtype(dtype, "deeponet_head", [&](auto zero) {
+    using T = decltype(zero);
+    PPSCI_LAUNCH(k_deeponet_head<T>, dim3(blocks), dim3(256), 0, stream, (const T*)b, (const T*)t, (const T*)bias, act,
+                 (const T*)label, (const T*)weight, (long long)n, n_features, coef, (T*)g_out, loss_acc, (T*)bbar, (T*)tbar,
+                 (T*)dbias);
+    CK(cudaGetLastError());
+    return 0;
+  });
 }
 
 extern "C" int ppsci_b200_sample_uniform(int32_t dtype, uint64_t seed, uint64_t offset, int64_t n, int32_t ndim, const double* lo,
@@ -1244,17 +1252,11 @@ extern "C" int ppsci_b200_sample_uniform(int32_t dtype, uint64_t seed, uint64_t 
   a.seed = seed;
   a.offset = offset;
   const unsigned blocks = (unsigned)((n + 255) / 256);
-  if (dtype == PPSCI_F64) {
-    auto k = k_sample_uniform<double>;
-    PPSCI_LAUNCH(k, dim3(blocks), dim3(256), 0, stream, a);
-  } else if (dtype == PPSCI_F32) {
-    auto k = k_sample_uniform<float>;
-    PPSCI_LAUNCH(k, dim3(blocks), dim3(256), 0, stream, a);
-  } else {
-    return fail("sample_uniform: bad dtype");
-  }
-  CK(cudaGetLastError());
-  return 0;
+  return with_dtype(dtype, "sample_uniform", [&](auto zero) {
+    PPSCI_LAUNCH(k_sample_uniform<decltype(zero)>, dim3(blocks), dim3(256), 0, stream, a);
+    CK(cudaGetLastError());
+    return 0;
+  });
 }
 
 extern "C" int ppsci_b200_adam_step(int32_t dtype, void* params, const void* grads, void* exp_avg, void* exp_avg_sq,
@@ -1263,19 +1265,13 @@ extern "C" int ppsci_b200_adam_step(int32_t dtype, void* params, const void* gra
   if (!params || !grads || !exp_avg || !exp_avg_sq || n <= 0 || step < 1) return fail("adam_step: bad arguments");
   const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
   const unsigned blocks = (unsigned)((n + 255) / 256);
-  if (dtype == PPSCI_F64) {
-    auto k = k_adam<double>;
-    PPSCI_LAUNCH(k, dim3(blocks), dim3(256), 0, stream, (double*)params, (const double*)grads, (double*)exp_avg,
-                 (double*)exp_avg_sq, (long long)n, lr, beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale);
-  } else if (dtype == PPSCI_F32) {
-    auto k = k_adam<float>;
-    PPSCI_LAUNCH(k, dim3(blocks), dim3(256), 0, stream, (float*)params, (const float*)grads, (float*)exp_avg,
-                 (float*)exp_avg_sq, (long long)n, lr, beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale);
-  } else {
-    return fail("adam_step: bad dtype");
-  }
-  CK(cudaGetLastError());
-  return 0;
+  return with_dtype(dtype, "adam_step", [&](auto zero) {
+    using T = decltype(zero);
+    PPSCI_LAUNCH(k_adam<T>, dim3(blocks), dim3(256), 0, stream, (T*)params, (const T*)grads, (T*)exp_avg, (T*)exp_avg_sq,
+                 (long long)n, lr, beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale);
+    CK(cudaGetLastError());
+    return 0;
+  });
 }
 
 extern "C" int ppsci_b200_adam_step_dev(int32_t dtype, void* params, void* grads, void* exp_avg, void* exp_avg_sq,
@@ -1283,17 +1279,11 @@ extern "C" int ppsci_b200_adam_step_dev(int32_t dtype, void* params, void* grads
                                         double weight_decay, int32_t zero_grads, void* stream) {
   if (!params || !grads || !exp_avg || !exp_avg_sq || !hyper_dev || n <= 0) return fail("adam_step_dev: bad arguments");
   const unsigned blocks = (unsigned)((n + 255) / 256);
-  if (dtype == PPSCI_F64) {
-    auto k = k_adam_dev<double>;
-    PPSCI_LAUNCH(k, dim3(blocks), dim3(256), 0, stream, (double*)params, (double*)grads, (double*)exp_avg,
-                 (double*)exp_avg_sq, (long long)n, hyper_dev, beta1, beta2, eps, weight_decay, (int)zero_grads);
-  } else if (dtype == PPSCI_F32) {
-    auto k = k_adam_dev<float>;
-    PPSCI_LAUNCH(k, dim3(blocks), dim3(256), 0, stream, (float*)params, (float*)grads, (float*)exp_avg,
-                 (float*)exp_avg_sq, (long long)n, hyper_dev, beta1, beta2, eps, weight_decay, (int)zero_grads);
-  } else {
-    return fail("adam_step_dev: bad dtype");
-  }
-  CK(cudaGetLastError());
-  return 0;
+  return with_dtype(dtype, "adam_step_dev", [&](auto zero) {
+    using T = decltype(zero);
+    PPSCI_LAUNCH(k_adam_dev<T>, dim3(blocks), dim3(256), 0, stream, (T*)params, (T*)grads, (T*)exp_avg, (T*)exp_avg_sq,
+                 (long long)n, hyper_dev, beta1, beta2, eps, weight_decay, (int)zero_grads);
+    CK(cudaGetLastError());
+    return 0;
+  });
 }

@@ -8,6 +8,9 @@
 // code is checked on the CPU (tests/test_jet_layouts.py).
 #pragma once
 
+#include <type_traits>
+#include <utility>
+
 #include "jet_math.h"
 #include "ppsci_b200.h"
 
@@ -37,7 +40,43 @@ struct SLay {
   PPSCI_HD static int n_dir(const JetLayout&) { return ND; }
   PPSCI_HD static int order(const JetLayout&, int d) { return d == 0 ? O0 : d == 1 ? O1 : d == 2 ? O2 : O3; }
   PPSCI_HD static int cbase(const JetLayout&, int d) { return 1 + (d > 0 ? O0 : 0) + (d > 1 ? O1 : 0) + (d > 2 ? O2 : 0); }
+  // J has this layout's directions (its channel bases follow from the orders)
+  PPSCI_HD static bool matches(const JetLayout& J) {
+    bool ok = J.n_dir == ND;
+    for (int d = 0; d < ND; ++d) ok = ok && J.dir_order[d] == order(J, d);
+    return ok;
+  }
 };
+
+// The compile-time layouts of the kernels: Navier-Stokes / Poisson in 2-D (Lay22) and 3-D (Lay222), a first-order time
+// and a second-order space direction (Lay12), values only (LayV), and the polarised biharmonic operator (Lay4444).
+using Lay22 = SLay<2, 2, 0, 0>;
+using Lay12 = SLay<1, 2, 0, 0>;
+using Lay222 = SLay<2, 2, 2, 0>;
+using LayV = SLay<0, 0, 0, 0>;
+using Lay4444 = SLay<4, 4, 4, 4>;
+
+// The layouts each kernel family is instantiated for; with_lay picks among them.
+template <class... Ls>
+struct LayList {};
+using ThinLays = LayList<Lay22, Lay12, Lay222, LayV>;           // kernels_thin.cuh
+using WgLays = LayList<Lay22, Lay12, Lay222, LayV, Lay4444>;    // kernels_wgmma.cuh
+
+// f(L{}) for the layout L of the list that J matches; false if none does
+template <class... Ls, class F>
+bool with_lay(LayList<Ls...>, const JetLayout& J, F&& f) {
+  return ((Ls::matches(J) ? (f(Ls{}), true) : false) || ...);
+}
+
+// f(std::integral_constant<int, V>{}) for V = v in 1..MAX; false if v is outside
+template <class F, int... I>
+bool with_int_(int v, F& f, std::integer_sequence<int, I...>) {
+  return ((v == I + 1 ? (f(std::integral_constant<int, I + 1>{}), true) : false) || ...);
+}
+template <int MAX, class F>
+bool with_int(int v, F&& f) {
+  return with_int_(v, f, std::make_integer_sequence<int, MAX>{});
+}
 
 // Channels 1..C-1 of y = act(z) for one element: channel c of z comes from ld(c), channel c of y goes to st(c, y_c).
 // s[1..Lay::KM] from act_coef / act_coef_p at z0; the caller handles channel 0 (y0).
@@ -78,19 +117,6 @@ PPSCI_HD T jet_adj(const JetLayout& J, const T (&s)[6], Ldz ldz, Ldyb ldyb, St s
       if (o < K) st(cb + o, zb[o]);
   }
   return jet_adj_z0<T, Lay::KM>(s, ldyb(0), sb);
-}
-
-enum { LAY_DYN = 0, LAY_22 = 1, LAY_12 = 2, LAY_222 = 3, LAY_VALUE = 4 };
-inline int pick_layout(const JetLayout& J, int act) {
-  if (act != PPSCI_ACT_TANH) return LAY_DYN;
-  auto is = [&](int n, int a, int b, int c) {
-    return J.n_dir == n && (n < 1 || J.dir_order[0] == a) && (n < 2 || J.dir_order[1] == b) && (n < 3 || J.dir_order[2] == c);
-  };
-  if (is(2, 2, 2, 0)) return LAY_22;
-  if (is(2, 1, 2, 0)) return LAY_12;
-  if (is(3, 2, 2, 2)) return LAY_222;
-  if (is(0, 0, 0, 0)) return LAY_VALUE;
-  return LAY_DYN;
 }
 
 }  // namespace ppsci

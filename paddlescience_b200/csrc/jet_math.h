@@ -42,6 +42,7 @@ enum ActId {
   ACT_STAN = 12,     // Stan (activation.py:28-46): tanh(z) (1 + beta z), beta per unit, 1 at start
   ACT_SWISH_B = 13,  // Swish (activation.py:49-58): z sigmoid(beta z), beta per layer, 1 at start
 };
+inline bool act_has_param(int act) { return act == ACT_STAN || act == ACT_SWISH_B; }
 
 template <typename T>
 PPSCI_HD T m_tanh(T x);

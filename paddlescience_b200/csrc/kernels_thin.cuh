@@ -3,7 +3,7 @@
 // The input layer (K = n_feat = 2..8) and the output layer (N = n_out = 1..8) are pure HBM streams: one pass
 // over a [C][Np][width] jet plane set.  The generic kernels in kernels_simt.cuh keep the channel structure at run
 // time (channel-indexed accumulators end up in local memory) and move 4 bytes per thread and instruction; these
-// specialisations fix the layout at compile time (SLay, jet_layout.cuh), move 16 bytes per thread and instruction along the
+// specialisations fix the layout at compile time (ThinLays, jet_layout.cuh), move 16 bytes per thread and instruction along the
 // hidden dimension, and evaluate the input seeds once per point into shared memory instead of once per thread.
 // Same arithmetic (jet_math.h); the generic kernels remain the fallback (fp64, runtime layouts, odd widths) and
 // the on-GPU cross-check (PPSCI_B200_NO_THINV=1).
@@ -14,34 +14,30 @@ namespace ppsci {
 namespace thin {
 
 constexpr int PB = 32;  // points per seed tile
-using Lay22 = SLay<2, 2, 0, 0>;
-using Lay12 = SLay<1, 2, 0, 0>;
-using Lay222 = SLay<2, 2, 2, 0>;
-using LayV = SLay<0, 0, 0, 0>;
 
 __device__ __forceinline__ float f4c(const float4& v, int t) { return t == 0 ? v.x : t == 1 ? v.y : t == 2 ? v.z : v.w; }
 
 // seeds of PB points -> shared memory  sS[pt][f][c]
-template <int CS, int KMAX>
-__device__ __forceinline__ void stage_seeds(const FirstArgs<float>& g, long long p0, float (*sS)[THIN_MAXF][CS]) {
+template <class L>
+__device__ __forceinline__ void stage_seeds(const FirstArgs<float>& g, long long p0, float (*sS)[THIN_MAXF][L::CS]) {
   for (int idx = threadIdx.x; idx < PB * g.nf; idx += blockDim.x) {
     const int pt = idx / g.nf, f = idx - pt * g.nf;
     const long long p = p0 + pt;
     const bool ok = p < g.Np;
-    produce_a<float, KMAX>(g.A, g.J, ok ? p : 0, f, ok, [&](int c, float v) {
-      if (c < CS) sS[pt][f][c] = v;
+    produce_a<float, L::KM>(g.A, g.J, ok ? p : 0, f, ok, [&](int c, float v) {
+      if (c < L::CS) sS[pt][f][c] = v;
     });
   }
 }
 
 // Z_1[c][p][n] = sum_f seed_c[p][f] W[f][n] (+ b[n] on the value channel).  Block = PB points x all columns.
-template <class L, int KMAX>
+template <class L>
 __global__ void __launch_bounds__(256) k_first_fwd_v(FirstArgs<float> g) {
   constexpr int CS = L::CS;
   __shared__ float sS[PB][THIN_MAXF][CS];
   const int tid = threadIdx.x;
   const long long p0 = (long long)blockIdx.x * PB;
-  stage_seeds<CS, KMAX>(g, p0, sS);
+  stage_seeds<L>(g, p0, sS);
   __syncthreads();
   const int lane4 = tid >> 6;
   for (int nq = tid & 63; nq * 4 < g.N; nq += 64) {
@@ -76,7 +72,7 @@ __global__ void __launch_bounds__(256) k_first_fwd_v(FirstArgs<float> g) {
 
 // dW_1[f][n] += sum_{c,p} seed_c[p][f] Zbar_1[c][p][n] ;  db_1[n] += sum_p Zbar_1[0][p][n]
 // grid (ceil(N / 256), ceil(Np / pts_per_block)), pts_per_block a multiple of PB.
-template <class L, int KMAX>
+template <class L>
 __global__ void __launch_bounds__(256) k_first_dw_v(FirstArgs<float> g) {
   constexpr int CS = L::CS;
   __shared__ float sS[PB][THIN_MAXF][CS];
@@ -94,7 +90,7 @@ __global__ void __launch_bounds__(256) k_first_dw_v(FirstArgs<float> g) {
     for (int t = 0; t < 4; ++t) acc[f][t] = 0.f;
   for (long long p0 = p_begin; p0 < p_end; p0 += PB) {
     __syncthreads();
-    stage_seeds<CS, KMAX>(g, p0, sS);
+    stage_seeds<L>(g, p0, sS);
     __syncthreads();
     if (!n_ok) continue;
     for (int pt = lane4; pt < PB; pt += 4) {
@@ -269,28 +265,4 @@ __global__ void __launch_bounds__(256) k_last_bwd_v(LastArgs<float> g) {
 }
 
 }  // namespace thin
-
-// layout x (n_out for the last-layer kernels) dispatch; `lay` from pick_layout(J, PPSCI_ACT_TANH), never LAY_DYN
-#define PPSCI_THIN_PICK_L(KERNEL, lay, kmax, kfn)                                                  \
-  switch (lay) {                                                                                   \
-    case LAY_22: kfn = thin::KERNEL<thin::Lay22, kmax>; break;                                  \
-    case LAY_12: kfn = thin::KERNEL<thin::Lay12, kmax>; break;                                  \
-    case LAY_222: kfn = thin::KERNEL<thin::Lay222, kmax>; break;                                \
-    default: kfn = thin::KERNEL<thin::LayV, kmax>;                                                 \
-  }
-#define PPSCI_THIN_PICK_LM_(KERNEL, LAY, m, kfn)                                                   \
-  switch (m) {                                                                                     \
-    case 1: kfn = thin::KERNEL<LAY, 1>; break;                                                     \
-    case 2: kfn = thin::KERNEL<LAY, 2>; break;                                                     \
-    case 3: kfn = thin::KERNEL<LAY, 3>; break;                                                     \
-    default: kfn = thin::KERNEL<LAY, 4>;                                                           \
-  }
-#define PPSCI_THIN_PICK_LM(KERNEL, lay, m, kfn)                                                    \
-  switch (lay) {                                                                                   \
-    case LAY_22: PPSCI_THIN_PICK_LM_(KERNEL, thin::Lay22, m, kfn); break;                       \
-    case LAY_12: PPSCI_THIN_PICK_LM_(KERNEL, thin::Lay12, m, kfn); break;                       \
-    case LAY_222: PPSCI_THIN_PICK_LM_(KERNEL, thin::Lay222, m, kfn); break;                     \
-    default: PPSCI_THIN_PICK_LM_(KERNEL, thin::LayV, m, kfn);                                      \
-  }
-
 }  // namespace ppsci

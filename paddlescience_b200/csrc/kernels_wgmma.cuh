@@ -1,5 +1,5 @@
 // kernels_wgmma.cuh — Hopper (sm_90a) tensor-core kernels for the fp32 layers (K a multiple of 32 up to 1024, N a
-// multiple of 32 up to 256) with one of the compile-time jet layouts: the forward  Z_l = act_jets(Z_{l-1}) W_l + b_l, the
+// multiple of 32 up to 256) with a jet layout of WgLays (jet_layout.cuh): the forward  Z_l = act_jets(Z_{l-1}) W_l + b_l, the
 // dx  Zbar_{l-1} = adj(Zbar_l W_l^T, Z_{l-1})  (k_wg_layer) and the weight gradient (k_wg_dw, further down).
 //
 // fp32-faithful contraction on TF32 tensor cores: every operand is split x = hi + lo with hi = rn_tf32(x), lo = x - hi
@@ -418,7 +418,6 @@ __host__ __device__ constexpr int dw_atoms(int C) { return (dw_ksteps(C) + 3) / 
 // widest column block in units of 32: two accumulators of BN / 2 registers each, beside the A fragments and the B
 // prefetch of a chunk, must fit in 255 registers without spilling
 __host__ __device__ constexpr int dw_maxq(int C) { return C <= 5 ? 4 : C <= 8 ? 2 : 1; }
-__host__ __device__ constexpr int dw_q(int C, int q) { return q < dw_maxq(C) ? q : dw_maxq(C); }
 // two stages of [hi | lo][atoms][BN rows x 128 bytes], 1024-byte aligned, then the db_l column sums, the A operand's
 // per-thread Z_{l-1} slots and the per-thread partial sums of the flushed accumulators (BN / 2 per thread)
 __host__ __device__ constexpr int dw_smem_bytes(int C, int bnq) {
@@ -669,86 +668,33 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_dw(WgDwArgs g) {
 
 }  // namespace wg
 
-// jet layouts of the wgmma kernels: the thin kernels' compile-time layouts and four fourth-order directions (the
-// polarised biharmonic operator)
-enum { WG_LAY_4444 = 16 };
-inline int wg_layout(const JetLayout& J) {
-  const int lay = pick_layout(J, PPSCI_ACT_TANH);
-  if (lay != LAY_DYN) return lay;
-  bool o4 = J.n_dir == 4;
-  for (int d = 0; d < J.n_dir; ++d) o4 = o4 && J.dir_order[d] == 4;
-  return o4 ? (int)WG_LAY_4444 : (int)LAY_DYN;
-}
 // a GEMM of contraction length K and N output columns on k_wg_layer
 inline int wg_kpad(int K) { return (K + wg::KCH - 1) / wg::KCH * wg::KCH; }
 inline bool wg_shape_ok(int K, int N) { return K % wg::KCH == 0 && K >= 32 && K <= 1024 && N % 32 == 0 && N >= 32 && N <= 256; }
-// fp32 layer l whose forward runs on k_wg_layer: one of the wgmma jet layouts, an activation without a trainable
-// parameter; layer 1 only as a dense first layer (its operand the caller's matrix, contraction padded to 32)
-inline bool wg_fwd_ok(const ppsci_plan_spec& s, int l, const JetLayout& J) {
-  if (s.dtype != PPSCI_F32 || s.gated) return false;
-  if (s.act == PPSCI_ACT_STAN || s.act == PPSCI_ACT_SWISH_B) return false;
-  if (wg_layout(J) == LAY_DYN) return false;
+// the plans whose layers may run on the wgmma kernels: fp32, not gated, an activation without a trainable parameter and
+// a jet layout of WgLays; which passes of which layers do is up to wg_fwd_ok / wg_dx_ok / wg_dw_ok
+inline bool wg_plan_ok(const ppsci_plan_spec& s, const JetLayout& J) {
+  return s.dtype == PPSCI_F32 && !s.gated && !act_has_param(s.act) && with_lay(WgLays{}, J, [](auto) {});
+}
+// forward of layer l on k_wg_layer; layer 1 only as a dense first layer (its operand the caller's matrix, contraction
+// padded to 32)
+inline bool wg_fwd_ok(const ppsci_plan_spec& s, int l) {
   if (l == 1) return s.dense_in && s.n_layers >= 2 && s.widths[0] % 4 == 0 && wg_shape_ok(wg_kpad(s.widths[0]), s.widths[1]);
   if (l < 2 || l > s.n_layers) return false;  // l == n_layers: a wide output layer
   return wg_shape_ok(s.widths[l - 1], s.widths[l]);
 }
 // dx through layer l (produces Zbar_{l-1} of hidden layer l - 1): gemm K = width of layer l, gemm N = width of layer l - 1
-inline bool wg_dx_ok(const ppsci_plan_spec& s, int l, const JetLayout& J) {
-  if (s.dtype != PPSCI_F32 || s.gated) return false;
-  if (s.act == PPSCI_ACT_STAN || s.act == PPSCI_ACT_SWISH_B) return false;
-  if (l < 2 || l > s.n_layers || wg_layout(J) == LAY_DYN) return false;
+inline bool wg_dx_ok(const ppsci_plan_spec& s, int l) {
+  if (l < 2 || l > s.n_layers) return false;
   return wg_shape_ok(s.widths[l], s.widths[l - 1]);
 }
 
 // dW of layer l: fan-in a multiple of 4, fan-out a multiple of 32 up to 256; the A operand is the activation jets of the
 // hidden layer below, or for a dense first layer the caller's matrix
-inline bool wg_dw_ok(const ppsci_plan_spec& s, int l, const JetLayout& J) {
-  if (s.dtype != PPSCI_F32 || s.gated) return false;
-  if (s.act == PPSCI_ACT_STAN || s.act == PPSCI_ACT_SWISH_B) return false;
-  if (l < 1 || (l == 1 && !s.dense_in) || l > s.n_layers || wg_layout(J) == LAY_DYN) return false;
+inline bool wg_dw_ok(const ppsci_plan_spec& s, int l) {
+  if (l < 1 || (l == 1 && !s.dense_in) || l > s.n_layers) return false;
   const int K = s.widths[l - 1], N = s.widths[l];
   return K % 4 == 0 && N % 32 == 0 && N >= 32 && N <= 256;
-}
-
-namespace wg {
-using Lay4444 = SLay<4, 4, 4, 4>;
-}
-// k_wg_dw instance for jet layout `lay` (wg_layout) and a column block of q x 32 columns (q <= dw_maxq(C)); layouts with
-// more channels instantiate only the narrower blocks
-#define PPSCI_WG_DW_PICK_(LAY, q)                                                                                \
-  ((q) == 4   ? wg::k_wg_dw<LAY, wg::dw_q(LAY::CS, 4)>                                                          \
-   : (q) == 3 ? wg::k_wg_dw<LAY, wg::dw_q(LAY::CS, 3)>                                                          \
-   : (q) == 2 ? wg::k_wg_dw<LAY, 2>                                                                             \
-              : wg::k_wg_dw<LAY, 1>)
-inline auto wg_dw_kernel(int lay, int q) -> void (*)(wg::WgDwArgs) {
-  switch (lay) {
-    case LAY_22: return PPSCI_WG_DW_PICK_(thin::Lay22, q);
-    case LAY_12: return PPSCI_WG_DW_PICK_(thin::Lay12, q);
-    case LAY_222: return PPSCI_WG_DW_PICK_(thin::Lay222, q);
-    case WG_LAY_4444: return PPSCI_WG_DW_PICK_(wg::Lay4444, q);
-    default: return PPSCI_WG_DW_PICK_(thin::LayV, q);
-  }
-}
-
-// k_wg_layer instance (DX: the dx variant) for jet layout `lay` and n output columns
-#define PPSCI_WG_PICK_(DX, LAY, n)                                                                               \
-  ((n) == 256   ? wg::k_wg_layer<LAY, 8, DX>                                                                    \
-   : (n) == 224 ? wg::k_wg_layer<LAY, 7, DX>                                                                    \
-   : (n) == 192 ? wg::k_wg_layer<LAY, 6, DX>                                                                    \
-   : (n) == 160 ? wg::k_wg_layer<LAY, 5, DX>                                                                    \
-   : (n) == 128 ? wg::k_wg_layer<LAY, 4, DX>                                                                    \
-   : (n) == 96  ? wg::k_wg_layer<LAY, 3, DX>                                                                    \
-   : (n) == 64  ? wg::k_wg_layer<LAY, 2, DX>                                                                    \
-                : wg::k_wg_layer<LAY, 1, DX>)
-template <bool DX>
-inline auto wg_layer_kernel(int lay, int n) -> void (*)(wg::WgArgs) {
-  switch (lay) {
-    case LAY_22: return PPSCI_WG_PICK_(DX, thin::Lay22, n);
-    case LAY_12: return PPSCI_WG_PICK_(DX, thin::Lay12, n);
-    case LAY_222: return PPSCI_WG_PICK_(DX, thin::Lay222, n);
-    case WG_LAY_4444: return PPSCI_WG_PICK_(DX, wg::Lay4444, n);
-    default: return PPSCI_WG_PICK_(DX, thin::LayV, n);
-  }
 }
 
 }  // namespace ppsci

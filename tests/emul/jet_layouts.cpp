@@ -1,5 +1,6 @@
 // Host harness of tests/test_jet_layouts.py: the per-element jet step (jet_fwd, jet_adj) of jet_layout.cuh through a
-// compile-time layout (SLay) or through the runtime layout (DynLay) of the same channel structure.
+// compile-time layout (SLay) or through the runtime layout (DynLay) of the same channel structure, and the layout
+// picker with_lay over the kernel families' layout lists.
 #include "jet_layout.cuh"
 
 using namespace ppsci;
@@ -7,6 +8,47 @@ using namespace ppsci;
 namespace {
 
 constexpr int MAXC = 32;
+
+// family 0: ThinLays, 1: WgLays, 2: the layouts of the jet-step test, i.e. those of every family, plus SLay<1, 2, 3, 4>
+// (every direction of a different order, which no kernel takes)
+template <class... A, class... B, class... C>
+LayList<A..., B..., C...> cat(LayList<A...>, LayList<B...>, LayList<C...>);
+using StepLays = decltype(cat(WgLays{}, ThinLays{}, LayList<SLay<1, 2, 3, 4>>{}));
+
+// f(L{}) for the i-th layout L of the list; false past its end
+template <class... Ls, class F>
+bool with_nth(LayList<Ls...>, int i, F&& f) {
+  int k = 0;
+  return ((k++ == i ? (f(Ls{}), true) : false) || ...);
+}
+template <class F>
+bool with_family(int family, int i, F&& f) {
+  return family == 0 ? with_nth(ThinLays{}, i, f) : family == 1 ? with_nth(WgLays{}, i, f) : with_nth(StepLays{}, i, f);
+}
+
+// direction count of layout L; its orders and channel bases -> orders[d], bases[d]
+template <class L>
+int describe(int* orders, int* bases) {
+  const JetLayout J{};
+  for (int d = 0; d < L::n_dir(J); ++d) {
+    orders[d] = L::order(J, d);
+    bases[d] = L::cbase(J, d);
+  }
+  return L::n_dir(J);
+}
+
+// The JetLayout of n_dir directions of the given orders, built as the engine builds it, independently of SLay's index math.
+JetLayout make_layout(int n_dir, const int* orders) {
+  JetLayout J{};
+  J.C = 1;
+  J.n_dir = n_dir;
+  for (int d = 0; d < PPSCI_MAX_DIR; ++d) {
+    J.dir_order[d] = d < n_dir ? orders[d] : 0;
+    J.dir_base[d] = J.C;
+    if (d < n_dir) J.C += orders[d];
+  }
+  return J;
+}
 
 // One element per row of z / yb ([n][MAXC], channels past the layout's C ignored).  Outputs y = act(z) jets and zb,
 // the adjoint of z, are [n][MAXC] too; channels the step does not write keep the sentinel the caller filled in.
@@ -32,20 +74,10 @@ void run(const JetLayout& J, int act, long long n, const double* z, const double
   }
 }
 
-// The JetLayout is built from the direction orders as the engine builds it, independently of SLay's index math.
-template <int O0, int O1, int O2, int O3>
-int dispatch(int dyn, int dbl, int ns_plus, int act, long long n, const double* z, const double* yb, double* y,
-             double* zb) {
-  using L = SLay<O0, O1, O2, O3>;
-  const int orders[4] = {O0, O1, O2, O3};
-  JetLayout J{};
-  J.C = 1;
-  for (int d = 0; d < 4 && orders[d] > 0; ++d) {
-    J.dir_order[d] = orders[d];
-    J.dir_base[d] = J.C;
-    J.C += orders[d];
-    J.n_dir = d + 1;
-  }
+template <class L>
+int step(int dyn, int dbl, int ns_plus, int act, long long n, const double* z, const double* yb, double* y, double* zb) {
+  int orders[4], bases[4];
+  const JetLayout J = make_layout(describe<L>(orders, bases), orders);
   using D = DynLay<L::KM>;
   constexpr int NS = L::KM;
   if (dbl) {
@@ -60,17 +92,29 @@ int dispatch(int dyn, int dbl, int ns_plus, int act, long long n, const double* 
 
 }  // namespace
 
-// lay: 0 Lay22, 1 Lay12, 2 Lay222, 3 LayV, 4 Lay4444 (the kernels' layouts), 5 SLay<1, 2, 3, 4> (every direction of a
-// different order).  dyn: DynLay instead of SLay.  ns_plus: act_coef with NS = KM + 1 instead of KM.  Returns C.
-extern "C" int jet_layout_step(int lay, int dyn, int dbl, int ns_plus, int act, long long n, const double* z,
+// Layout i of family (see above): returns its direction count and writes its orders and channel bases, -1 past the end.
+extern "C" int jet_layout_info(int family, int i, int* orders, int* bases) {
+  int nd = -1;
+  with_family(family, i, [&](auto lay) { nd = describe<decltype(lay)>(orders, bases); });
+  return nd;
+}
+
+// The jet step through layout i of family 2.  dyn: DynLay instead of SLay.  ns_plus: act_coef with NS = KM + 1 instead
+// of KM.  Returns C, -1 past the end of the list.
+extern "C" int jet_layout_step(int i, int dyn, int dbl, int ns_plus, int act, long long n, const double* z,
                                const double* yb, double* y, double* zb) {
-  switch (lay) {
-    case 0: return dispatch<2, 2, 0, 0>(dyn, dbl, ns_plus, act, n, z, yb, y, zb);
-    case 1: return dispatch<1, 2, 0, 0>(dyn, dbl, ns_plus, act, n, z, yb, y, zb);
-    case 2: return dispatch<2, 2, 2, 0>(dyn, dbl, ns_plus, act, n, z, yb, y, zb);
-    case 3: return dispatch<0, 0, 0, 0>(dyn, dbl, ns_plus, act, n, z, yb, y, zb);
-    case 4: return dispatch<4, 4, 4, 4>(dyn, dbl, ns_plus, act, n, z, yb, y, zb);
-    case 5: return dispatch<1, 2, 3, 4>(dyn, dbl, ns_plus, act, n, z, yb, y, zb);
-    default: return -1;
-  }
+  int C = -1;
+  with_family(2, i, [&](auto lay) { C = step<decltype(lay)>(dyn, dbl, ns_plus, act, n, z, yb, y, zb); });
+  return C;
+}
+
+// with_lay over family 0 or 1 for the JetLayout of n_dir directions of the given orders: the direction count, orders and
+// channel bases of the layout it picks, -1 if it picks none.
+extern "C" int jet_layout_pick(int family, int n_dir, const int* orders, int* orders_out, int* bases_out) {
+  const JetLayout J = make_layout(n_dir, orders);
+  int nd = -1;
+  auto f = [&](auto lay) { nd = describe<decltype(lay)>(orders_out, bases_out); };
+  if (family == 0) with_lay(ThinLays{}, J, f);
+  if (family == 1) with_lay(WgLays{}, J, f);
+  return nd;
 }
