@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import math
 from collections import OrderedDict
-from typing import Dict, List, Tuple, Union
+from typing import Dict, Tuple, Union
 
 import torch
 from torch import nn
@@ -17,6 +17,7 @@ from torch import nn
 from ..engine.compiler import NetSpec, compile_residuals
 from . import activation as act_mod
 from . import base
+from .mlp import Reparam, hidden_sizes, stack_offsets
 
 _TORCH_ACT = {
     "tanh": torch.tanh, "sin": torch.sin, "cos": torch.cos, "sigmoid": torch.sigmoid, "silu": torch.nn.functional.silu,
@@ -24,88 +25,6 @@ _TORCH_ACT = {
     "elu": torch.nn.functional.elu, "selu": torch.nn.functional.selu, "leaky_relu": torch.nn.functional.leaky_relu,
     "siren": lambda t: torch.sin(30.0 * t),
 }
-
-
-def _hidden(num_layers, hidden_size) -> List[int]:
-    if isinstance(hidden_size, (tuple, list)):
-        if num_layers is not None:
-            raise ValueError("num_layers should be None when hidden_size is specified")
-        return [int(h) for h in hidden_size]
-    if not isinstance(num_layers, int):
-        raise ValueError("num_layers should be an int when hidden_size is an int")
-    return [int(hidden_size)] * num_layers
-
-
-class _SubnetReparam:
-    """Host-side reparametrisation of one sub-network around the unchanged native calls, exactly as ``arch.MLP`` does it:
-    ``weight_norm`` (WeightNormLinear on the hidden layers, mlp.py:31-53, 234-246: W = g V / ||V||_col, stored as V in the
-    weight slot and g behind the model's other parameters) and ``skip_connection`` (mlp.py:281-296 as executed: the
-    pre-activation of every even hidden layer i >= 2 is doubled, i.e. effective 2 W_i, 2 b_i)."""
-
-    def __init__(self, widths, lo: int, weight_norm: bool, skip: bool, g_off: int):
-        self.shapes = list(zip(widths[:-1], widths[1:]))
-        self.lo = lo
-        self.weight_norm, self.skip = bool(weight_norm), bool(skip)
-        self.w_off, self.b_off, off = [], [], 0
-        for a, b in self.shapes:
-            self.w_off.append(off)
-            off += a * b
-            self.b_off.append(off)
-            off += b
-        self.n = off
-        n_hidden = len(self.shapes) - 1
-        self.g_off = []  # absolute offsets of the gain vectors of the weight-normalised hidden layers
-        for _, b in (self.shapes[:-1] if self.weight_norm else []):
-            self.g_off.append(g_off)
-            g_off += b
-        self.g_end = g_off
-        self.skip_layers = [i for i in range(n_hidden) if self.skip and i % 2 == 0 and i >= 2]
-        self.active = self.weight_norm or bool(self.skip_layers)
-        self.eff = self.eff_grad = None
-
-    def params(self, flat: torch.Tensor) -> torch.Tensor:
-        raw = flat.data[self.lo: self.lo + self.n]
-        if not self.active:
-            return raw
-        if self.eff is None or self.eff.device != raw.device or self.eff.dtype != raw.dtype:
-            self.eff, self.eff_grad = torch.empty_like(raw), torch.zeros_like(raw)
-        with torch.no_grad():
-            self.eff.copy_(raw)
-            for i, (a, b) in enumerate(self.shapes[:-1]):
-                w = self.eff[self.w_off[i]: self.w_off[i] + a * b].view(a, b)
-                if self.weight_norm:
-                    g = flat.data[self.g_off[i]: self.g_off[i] + b]
-                    w.mul_(g / w.norm(p=2, dim=0, keepdim=True))
-                if i in self.skip_layers:
-                    self.eff[self.w_off[i]: self.b_off[i] + b].mul_(2.0)
-        return self.eff
-
-    def grads(self, flat: torch.Tensor) -> torch.Tensor:
-        return self.eff_grad if self.active else flat.grad[self.lo: self.lo + self.n]
-
-    def finish(self, flat: torch.Tensor):
-        """Chain rule from the effective-weight gradients into (V, g, b); clears the staging buffer."""
-        if not self.active:
-            return
-        with torch.no_grad():
-            eg = self.eff_grad
-            for i in self.skip_layers:
-                a, b = self.shapes[i]
-                eg[self.w_off[i]: self.b_off[i] + b].mul_(2.0)
-            gr = flat.grad[self.lo: self.lo + self.n]
-            gr += eg
-            if self.weight_norm:
-                for i, (a, b) in enumerate(self.shapes[:-1]):
-                    sl = slice(self.w_off[i], self.w_off[i] + a * b)
-                    v = flat.data[self.lo: self.lo + self.n][sl].view(a, b)
-                    g = flat.data[self.g_off[i]: self.g_off[i] + b]
-                    dw = eg[sl].view(a, b)
-                    norm = v.norm(p=2, dim=0, keepdim=True)
-                    dot = (dw * v).sum(dim=0, keepdim=True)
-                    dv = (g / norm) * (dw - v * (dot / (norm * norm)))
-                    gr[sl].view(a, b).add_(dv - dw)
-                    flat.grad[self.g_off[i]: self.g_off[i] + b] += (dot / norm).view(-1)
-            eg.zero_()
 
 
 class DeepONet(base.Arch):
@@ -148,43 +67,49 @@ class DeepONet(base.Arch):
                                           "supported by arch.MLP only")
             if a == "swish":
                 act_mod.warn_fixed_swish()
-        bw = [self.num_loc] + _hidden(branch_num_layers, branch_hidden_size) + [self.num_features]
-        tw = [1] + _hidden(trunk_num_layers, trunk_hidden_size) + [self.num_features]
+        bw = [self.num_loc] + hidden_sizes(branch_num_layers, branch_hidden_size) + [self.num_features]
+        tw = [1] + hidden_sizes(trunk_num_layers, trunk_hidden_size) + [self.num_features]
         feats = tuple(f"f{i}" for i in range(self.num_features))
         self._branch = NetSpec((u_key,), feats, [], [], [], bw, self.branch_activation, dense_in=True)
         self._trunk = NetSpec((y_key,), feats, [0], [0], [0.0], tw, self.trunk_activation)
-        nb, nt = self._branch.n_params, self._trunk.n_params
-        self._b_rng = (0, nb)
-        t0 = (nb + 3) // 4 * 4
-        self._t_rng = (t0, t0 + nt)
-        self._bias_off = (t0 + nt + 3) // 4 * 4
-        g0 = self._bias_off + (1 if self.use_bias else 0)
-        self._rb = _SubnetReparam(bw, 0, branch_weight_norm, branch_skip_connection, g0)
-        self._rt = _SubnetReparam(tw, t0, trunk_weight_norm, trunk_skip_connection, self._rb.g_end)
-        self.flat = nn.Parameter(torch.zeros(self._rt.g_end, dtype=dtype))
+        t0 = (self._branch.n_params + 3) // 4 * 4
+        self._bias_off = (t0 + self._trunk.n_params + 3) // 4 * 4
+        off = self._bias_off + (1 if self.use_bias else 0)  # the gains behind b: the branch net's, then the trunk net's
+        subnets, self._staged = [], []
+        for widths, lo, wn, skip in ((bw, 0, branch_weight_norm, branch_skip_connection),
+                                     (tw, t0, trunk_weight_norm, trunk_skip_connection)):
+            shapes = list(zip(widths[:-1], widths[1:]))
+            w_off, b_off, n = stack_offsets(shapes, 0)
+            g_off = {}
+            for i in range(len(shapes) - 1) if wn else ():  # WeightNormLinear on the hidden layers (mlp.py:234-246)
+                g_off[i], off = off, off + shapes[i][1]
+            # skip_connection as in arch.MLP: the pre-activation of every even hidden layer i >= 2 is doubled (2 W_i, 2 b_i)
+            doubled = {i: (w_off[i], b_off[i] + shapes[i][1]) for i in range(2, len(shapes) - 1, 2)} if skip else {}
+            subnets.append(Reparam(shapes, lo, n, g_off, wn, doubled))
+            if wn or doubled:
+                self._staged.append(subnets[-1])
+        self._rb, self._rt = subnets
+        self._eff = self._eff_grad = None  # staging buffers laid out like flat, allocated on first use
+        self.flat = nn.Parameter(torch.zeros(off, dtype=dtype))
         self.reset_parameters()
         self._plans = None
 
     # ---- parameters ------------------------------------------------------------------------------
-    def _layers(self, which: str):
-        net, (lo, _) = (self._branch, self._b_rng) if which == "branch_net" else (self._trunk, self._t_rng)
-        off = lo
-        n = len(net.widths) - 1
-        for i, (a, b) in enumerate(zip(net.widths[:-1], net.widths[1:])):
-            name = f"{which}.linears.{i}" if i < n - 1 else f"{which}.last_fc"
-            yield name, (a, b), off, off + a * b
-            off += a * b + b
+    def _layers(self):
+        """(sub-network, layer index, reference name, (in, out), weight offset, bias offset) of every layer, branch first."""
+        for which, r in (("branch_net", self._rb), ("trunk_net", self._rt)):
+            for i, (a, b) in enumerate(r.shapes):
+                name = f"{which}.linears.{i}" if i < len(r.shapes) - 1 else f"{which}.last_fc"
+                yield r, i, name, (a, b), r.lo + r.w_off[i], r.lo + r.b_off[i]
 
     def reset_parameters(self):
         """Xavier-uniform weights, zero biases, b = 0 (Paddle nn.Linear defaults; deeponet.py:121-125)."""
         with torch.no_grad():
             self.flat.data.zero_()
-            for which in ("branch_net", "trunk_net"):
-                for _, (a, b), w0, w1 in self._layers(which):
-                    lim = math.sqrt(6.0 / (a + b))
-                    self.flat.data[w0:w1] = ((torch.rand(a * b, dtype=torch.float64) * 2 - 1) * lim).to(self.flat.dtype)
-            for r in (self._rb, self._rt):  # WeightNormLinear._init_weights: g = 1
-                for i, (a, b) in enumerate(r.shapes[:-1] if r.weight_norm else []):
+            for r, i, _, (a, b), w0, w1 in self._layers():
+                lim = math.sqrt(6.0 / (a + b))
+                self.flat.data[w0:w1] = ((torch.rand(a * b, dtype=torch.float64) * 2 - 1) * lim).to(self.flat.dtype)
+                if i in r.g_off:  # WeightNormLinear._init_weights: g = 1
                     self.flat.data[r.g_off[i]: r.g_off[i] + b] = 1
 
     @property
@@ -193,14 +118,13 @@ class DeepONet(base.Arch):
 
     def state_dict(self, *args, **kwargs):  # reference-style keys
         out = OrderedDict()
-        for which, r in (("branch_net", self._rb), ("trunk_net", self._rt)):
-            for i, (name, (a, b), w0, w1) in enumerate(self._layers(which)):
-                if r.weight_norm and i < len(r.g_off):  # WeightNormLinear: weight_v / weight_g (mlp.py:31-53)
-                    out[f"{name}.weight_v"] = self.flat.data[w0:w1].view(a, b).detach().clone()
-                    out[f"{name}.weight_g"] = self.flat.data[r.g_off[i]: r.g_off[i] + b].detach().clone()
-                else:
-                    out[f"{name}.weight"] = self.flat.data[w0:w1].view(a, b).detach().clone()
-                out[f"{name}.bias"] = self.flat.data[w1: w1 + b].detach().clone()
+        for r, i, name, (a, b), w0, w1 in self._layers():
+            if i in r.g_off:  # WeightNormLinear: weight_v / weight_g (mlp.py:31-53)
+                out[f"{name}.weight_v"] = self.flat.data[w0:w1].view(a, b).detach().clone()
+                out[f"{name}.weight_g"] = self.flat.data[r.g_off[i]: r.g_off[i] + b].detach().clone()
+            else:
+                out[f"{name}.weight"] = self.flat.data[w0:w1].view(a, b).detach().clone()
+            out[f"{name}.bias"] = self.flat.data[w1: w1 + b].detach().clone()
         if self.use_bias:
             out["b"] = self.flat.data[self._bias_off: self._bias_off + 1].detach().clone()
         return out
@@ -208,17 +132,16 @@ class DeepONet(base.Arch):
     def load_state_dict(self, state_dict, strict: bool = True):
         missing = []
         with torch.no_grad():
-            for which, r in (("branch_net", self._rb), ("trunk_net", self._rt)):
-                for i, (name, (a, b), w0, w1) in enumerate(self._layers(which)):
-                    wn = r.weight_norm and i < len(r.g_off)
-                    slots = [(f"{name}.weight_v" if wn else f"{name}.weight", w0, w1), (f"{name}.bias", w1, w1 + b)]
-                    if wn:
-                        slots.append((f"{name}.weight_g", r.g_off[i], r.g_off[i] + b))
-                    for key, lo, hi in slots:
-                        if key not in state_dict:
-                            missing.append(key)
-                            continue
-                        self.flat.data[lo:hi] = torch.as_tensor(state_dict[key]).reshape(-1).to(self.flat.dtype).to(self.flat.device)
+            for r, i, name, (a, b), w0, w1 in self._layers():
+                wn = i in r.g_off
+                slots = [(f"{name}.weight_v" if wn else f"{name}.weight", w0, w1), (f"{name}.bias", w1, w1 + b)]
+                if wn:
+                    slots.append((f"{name}.weight_g", r.g_off[i], r.g_off[i] + b))
+                for key, lo, hi in slots:
+                    if key not in state_dict:
+                        missing.append(key)
+                        continue
+                    self.flat.data[lo:hi] = torch.as_tensor(state_dict[key]).reshape(-1).to(self.flat.dtype).to(self.flat.device)
             if self.use_bias:
                 if "b" in state_dict:
                     self.flat.data[self._bias_off] = float(torch.as_tensor(state_dict["b"]).reshape(-1)[0])
@@ -239,13 +162,38 @@ class DeepONet(base.Arch):
                                 for net in (self._branch, self._trunk))
         return self._plans
 
+    def _sub_params(self):
+        """Effective [W | b] of the branch and the trunk net: slices of ``flat``, or of the staging buffer for a
+        sub-network that ``*_weight_norm`` / ``*_skip_connection`` reparametrise."""
+        flat = self.flat.data
+        if self._staged and (self._eff is None or self._eff.device != flat.device or self._eff.dtype != flat.dtype):
+            self._eff, self._eff_grad = torch.empty_like(flat), torch.zeros_like(flat)
+        with torch.no_grad():
+            for r in self._staged:
+                r.fill(flat, self._eff[r.lo: r.lo + r.n])
+        return tuple((self._eff if r in self._staged else flat)[r.lo: r.lo + r.n] for r in (self._rb, self._rt))
+
+    def _sub_grads(self):
+        """Buffers the native calls accumulate the branch and the trunk weight gradients into (layout of ``_sub_params``)."""
+        return tuple((self._eff_grad if r in self._staged else self.flat.grad)[r.lo: r.lo + r.n]
+                     for r in (self._rb, self._rt))
+
+    def _finish_sub_grads(self):
+        """Chain rule of the reparametrised sub-networks into ``flat.grad``; clears the staging buffer."""
+        with torch.no_grad():
+            for r in self._staged:
+                eg = self._eff_grad[r.lo: r.lo + r.n]
+                r.chain(self.flat.data, self.flat.grad, eg)
+                eg.zero_()
+
     def _features(self, x: Dict[str, torch.Tensor]):
         pb, pt = self._get_plans()
         dt = self.flat.dtype
         u = x[self.u_key].to(dt)
         y = x[self.y_key].to(dt)
-        b = pb.forward({self.u_key: u}, self._rb.params(self.flat), want_jets=True, want_residuals=False)[0][0]
-        t = pt.forward({self.y_key: y}, self._rt.params(self.flat), want_jets=True, want_residuals=False)[0][0]
+        pbr, ptr_ = self._sub_params()
+        b = pb.forward({self.u_key: u}, pbr, want_jets=True, want_residuals=False)[0][0]
+        t = pt.forward({self.y_key: y}, ptr_, want_jets=True, want_residuals=False)[0][0]
         return u, y, b, t
 
     def _combine(self, b: torch.Tensor, t: torch.Tensor, bias) -> torch.Tensor:
@@ -304,8 +252,8 @@ class DeepONet(base.Arch):
         coef = float(loss_fn.weight_of(key) if hasattr(loss_fn, "weight_of") else 1.0) * (1.0 / n if red == "mean" else 1.0)
         pb, pt = self._get_plans()
         lib = pb.lib
-        pbr, ptr_ = self._rb.params(flat), self._rt.params(flat)  # effective [W | b] under weight_norm / skip_connection
-        gbr, gtr = self._rb.grads(flat), self._rt.grads(flat)
+        pbr, ptr_ = self._sub_params()  # effective [W | b] under weight_norm / skip_connection
+        gbr, gtr = self._sub_grads()
         loss_acc = torch.zeros(1, dtype=torch.float64, device=dev)
         bias = flat.data[self._bias_off: self._bias_off + 1] if self.use_bias else None
         dbias = flat.grad[self._bias_off: self._bias_off + 1] if self.use_bias else None
@@ -331,6 +279,5 @@ class DeepONet(base.Arch):
             lib.check(rc, "deeponet_head")
             pb.values_bwd_kept(pbr, gbr, bbar)  # bbar / tbar hold dL/d(branch), dL/d(trunk)
             pt.values_bwd_kept(ptr_, gtr, tbar)
-        self._rb.finish(flat)
-        self._rt.finish(flat)
+        self._finish_sub_grads()
         return {key: loss_acc[0].to(dt)}

@@ -27,6 +27,88 @@ from . import activation as act_mod
 from . import base
 
 
+def hidden_sizes(num_layers: Optional[int], hidden_size) -> List[int]:
+    """Widths of the hidden layers from the reference's ``(num_layers, hidden_size)`` pair (mlp.py:203-218)."""
+    if isinstance(hidden_size, (tuple, list)):
+        if num_layers is not None:
+            raise ValueError("num_layers should be None when hidden_size is specified")
+        return [int(h) for h in hidden_size]
+    if not isinstance(num_layers, int):
+        raise ValueError("num_layers should be an int when hidden_size is an int")
+    return [int(hidden_size)] * num_layers
+
+
+def stack_offsets(shapes, off: int):
+    """Weight and bias offsets of linear layers stored back to back from ``off`` as [W_1 (in,out) | b_1 | W_2 | ...],
+    and the offset behind the last bias."""
+    w_off, b_off = [], []
+    for a, b in shapes:
+        w_off.append(off)
+        off += a * b
+        b_off.append(off)
+        off += b
+    return w_off, b_off, off
+
+
+class Reparam:
+    """Host-side reparametrisation of a stack of linear layers around the unchanged native calls: the effective
+    [W | b] the kernels read, and the chain rule of their gradient back into the stored parameters.
+
+    The stack is stored as [W_1 (in,out) | b_1 | W_2 | ...] from ``flat[lo]``; the kernels read ``flat[lo: lo + n]``
+    (n may reach past the last bias: what lies there passes through) from a staging buffer of length n.  ``w_off`` /
+    ``b_off`` and the ranges of ``skip_layers`` are offsets from ``lo``, the gain offsets ``g_off`` are offsets into
+    ``flat``.  A factored layer i keeps V_i in its weight slot and a gain vector g_i at ``g_off[i]``: its effective
+    weight is W_i = g_i V_i / ||V_i||_col under ``weight_norm`` (WeightNormLinear, mlp.py:31-53) and W_i = g_i V_i
+    otherwise (RandomWeightFactorization, mlp.py:56-92).  ``skip_layers`` maps every hidden layer whose skip connection
+    fires to the [start, stop) range the kernels read at twice its stored value."""
+
+    def __init__(self, shapes, lo: int, n: int, g_off: Dict[int, int], weight_norm: bool,
+                 skip_layers: Dict[int, Tuple[int, int]]):
+        self.shapes, self.lo, self.n = shapes, lo, n
+        self.w_off, self.b_off, _ = stack_offsets(shapes, 0)
+        self.g_off, self.weight_norm, self.skip_layers = g_off, bool(weight_norm), skip_layers
+
+    def weight(self, flat: torch.Tensor, i: int) -> torch.Tensor:
+        """Effective weight [in, out] of factored layer i."""
+        a, b = self.shapes[i]
+        o = self.lo + self.w_off[i]
+        v = flat[o: o + a * b].view(a, b)
+        g = flat[self.g_off[i]: self.g_off[i] + b]
+        return v * (g / v.norm(p=2, dim=0, keepdim=True) if self.weight_norm else g)
+
+    def fill(self, flat: torch.Tensor, eff: torch.Tensor):
+        """Write the effective parameters of ``flat[lo: lo + n]`` into ``eff``."""
+        eff.copy_(flat[self.lo: self.lo + self.n])
+        for i in self.g_off:
+            a, b = self.shapes[i]
+            eff[self.w_off[i]: self.w_off[i] + a * b].view(a, b).copy_(self.weight(flat, i))
+        for lo, hi in self.skip_layers.values():
+            eff[lo:hi].mul_(2.0)
+
+    def chain(self, flat: torch.Tensor, grad: torch.Tensor, eff_grad: torch.Tensor):
+        """Add to ``grad`` the gradient w.r.t. the stored parameters, given ``eff_grad``, the gradient w.r.t. the
+        effective ones (left scaled in the doubled ranges)."""
+        for lo, hi in self.skip_layers.values():
+            eff_grad[lo:hi].mul_(2.0)  # d/dW = 2 d/dW_eff
+        sub, gsub = flat[self.lo: self.lo + self.n], grad[self.lo: self.lo + self.n]
+        gsub += eff_grad  # biases and plain layers pass through; the V parts are fixed below
+        for i, go in self.g_off.items():
+            a, b = self.shapes[i]
+            sl = slice(self.w_off[i], self.w_off[i] + a * b)
+            v = sub[sl].view(a, b)
+            g = flat[go: go + b]
+            dw = eff_grad[sl].view(a, b)
+            if not self.weight_norm:  # W = g * V  ->  dV = g * dW,  dg = sum_in V * dW
+                gsub[sl].view(a, b).add_(g * dw - dw)
+                grad[go: go + b] += (v * dw).sum(dim=0)
+                continue
+            norm = v.norm(p=2, dim=0, keepdim=True)
+            dot = (dw * v).sum(dim=0, keepdim=True)  # [1, out]
+            dv = (g / norm) * (dw - v * (dot / (norm * norm)))
+            gsub[sl].view(a, b).add_(dv - dw)  # replace the pass-through dW by dV
+            grad[go: go + b] += (dot / norm).view(-1)
+
+
 class _LinearView:
     """View of one layer inside the flat parameter buffer."""
 
@@ -37,14 +119,11 @@ class _LinearView:
     @property
     def weight(self) -> torch.Tensor:
         """Effective weight [in, out] (a view for plain layers, g * V / ||V||_col for weight-normalised ones)."""
+        if self._owner._wn_layer(self._index):
+            return self._owner._reparam.weight(self._owner.flat.data, self._index)
         a, b = self._owner._shapes[self._index]
         off = self._owner._w_off[self._index]
-        v = self._owner.flat.data[off: off + a * b].view(a, b)
-        if self._owner._wn_layer(self._index):
-            if self._owner.random_weight:
-                return v * self.weight_g
-            return v * (self.weight_g / v.norm(p=2, dim=0, keepdim=True))
-        return v
+        return self._owner.flat.data[off: off + a * b].view(a, b)
 
     @property
     def weight_v(self) -> torch.Tensor:
@@ -123,16 +202,9 @@ class MLP(base.Arch):
         self.input_keys = tuple(input_keys)
         self.output_keys = tuple(output_keys)
         self.periods = dict(periods) if periods else None
-        if isinstance(hidden_size, (tuple, list)):
-            if num_layers is not None:
-                raise ValueError("num_layers should be None when hidden_size is specified")
-            hidden = [int(h) for h in hidden_size]
-        elif isinstance(hidden_size, int):
-            if not isinstance(num_layers, int):
-                raise ValueError("num_layers should be an int when hidden_size is an int")
-            hidden = [hidden_size] * num_layers
-        else:
+        if not isinstance(hidden_size, (tuple, list, int)):
             raise ValueError(f"hidden_size should be list of int or int, but got {type(hidden_size)}")
+        hidden = hidden_sizes(num_layers, hidden_size)
         self.weight_norm = bool(weight_norm)
         self.fourier = dict(fourier) if fourier else None
         if self.fourier:
@@ -192,13 +264,7 @@ class MLP(base.Arch):
             if len(set(hidden)) != 1:
                 raise ValueError("ModifiedMLP takes one hidden_size for all layers")
             self._shapes += [(widths[0], hidden[0])] * 2
-        self._w_off, self._b_off = [], []
-        off = 0
-        for a, b in self._shapes:
-            self._w_off.append(off)
-            off += a * b
-            self._b_off.append(off)
-            off += b
+        self._w_off, self._b_off, off = stack_offsets(self._shapes, 0)
         self._alpha_off, self._n_blocks = off, 0
         if self._gated == 2:  # PirateNetBlock.alpha, one trainable scalar per block (mlp.py:592-597), behind the embeddings
             self._n_blocks = len(hidden) // 3
@@ -237,6 +303,7 @@ class MLP(base.Arch):
         # gate): the next linear layer sees 2 y, i.e. its weight (not its bias) is doubled.
         self.skip_connection = bool(skip_connection)
         self._skip_layers = [i for i in range(len(hidden)) if self.skip_connection and i % 2 == 0 and i >= 2]
+        self._reparam = Reparam(self._shapes, 0, self._n_eff, self._g_off, self.weight_norm, self._skip_slices())
         # the engine reads effective weights from a staging buffer [W0 | b0 (fourier) | reparametrised linear layers]
         self._has_eff = bool(self.weight_norm or self.random_weight or self.fourier or self._skip_layers)
         if self._has_eff:
@@ -293,15 +360,15 @@ class MLP(base.Arch):
         return self.weight_norm and i != self._n_hidden  # hidden layers (and the gated networks' embed_u / embed_v)
 
     def _skip_slices(self):
-        """(start, stop) ranges of the staging buffer that the reference's skip connection doubles."""
-        out = []
+        """Skip layer i -> the (start, stop) range of the staging buffer that the reference's skip connection doubles."""
+        out = {}
         for i in self._skip_layers:
             if self._gated:  # the layer BEHIND hidden layer i reads 2 y: its weight
                 a, b = self._shapes[i + 1]
-                out.append((self._w_off[i + 1], self._w_off[i + 1] + a * b))
+                out[i] = (self._w_off[i + 1], self._w_off[i + 1] + a * b)
             else:  # the pre-activation of hidden layer i is doubled: W_i and b_i (contiguous)
                 a, b = self._shapes[i]
-                out.append((self._w_off[i], self._b_off[i] + b))
+                out[i] = (self._w_off[i], self._b_off[i] + b)
         return out
 
     def engine_params(self) -> torch.Tensor:
@@ -310,17 +377,7 @@ class MLP(base.Arch):
         if not self._has_eff:
             return self.flat.data
         with torch.no_grad():
-            lin = self._eff[self._f_n0: self._f_n0 + self._n_eff]
-            lin.copy_(self.flat.data[: self._n_eff])
-            for i, (a, b) in enumerate(self._shapes):
-                if not self._wn_layer(i):
-                    continue
-                v = self.flat.data[self._w_off[i]: self._w_off[i] + a * b].view(a, b)
-                g = self.flat.data[self._g_off[i]: self._g_off[i] + b]
-                scale = g if self.random_weight else g / v.norm(p=2, dim=0, keepdim=True)
-                lin[self._w_off[i]: self._w_off[i] + a * b].view(a, b).copy_(v * scale)
-            for lo, hi in self._skip_slices():
-                lin[lo:hi].mul_(2.0)
+            self._reparam.fill(self.flat.data, self._eff[self._f_n0:])
             if self.fourier:
                 nf, dh = self._f_shape
                 k = self.fourier_kernel
@@ -346,26 +403,7 @@ class MLP(base.Arch):
             return
         with torch.no_grad():
             gr = self.flat.grad
-            lin_g = self._eff_grad[self._f_n0: self._f_n0 + self._n_eff]
-            for lo, hi in self._skip_slices():
-                lin_g[lo:hi].mul_(2.0)  # d/dW = 2 d/dW_eff
-            gr[: self._n_eff] += lin_g  # biases and plain layers pass through; the V parts are fixed below
-            for i, (a, b) in enumerate(self._shapes):
-                if not self._wn_layer(i):
-                    continue
-                sl = slice(self._w_off[i], self._w_off[i] + a * b)
-                v = self.flat.data[sl].view(a, b)
-                g = self.flat.data[self._g_off[i]: self._g_off[i] + b]
-                dw = lin_g[sl].view(a, b)
-                if self.random_weight:  # W = g * V  ->  dV = g * dW,  dg = sum_in V * dW
-                    gr[sl].view(a, b).add_(g * dw - dw)
-                    gr[self._g_off[i]: self._g_off[i] + b] += (v * dw).sum(dim=0)
-                    continue
-                norm = v.norm(p=2, dim=0, keepdim=True)
-                dot = (dw * v).sum(dim=0, keepdim=True)  # [1, out]
-                dv = (g / norm) * (dw - v * (dot / (norm * norm)))
-                gr[sl].view(a, b).add_(dv - dw)  # replace the pass-through dW by dV
-                gr[self._g_off[i]: self._g_off[i] + b] += (dot / norm).view(-1)
+            self._reparam.chain(self.flat.data, gr, self._eff_grad[self._f_n0:])
             if self.fourier:  # the tied kernel takes the sum of both halves; the constant bias [pi/2 | 0] takes none
                 nf, dh = self._f_shape
                 dw0 = self._eff_grad[: nf * 2 * dh].view(nf, 2 * dh)
