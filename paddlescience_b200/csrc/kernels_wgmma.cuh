@@ -10,14 +10,17 @@
 // an H100 80GB HBM3 (400 W power limit), cfg3 (6 x 256): one shared accumulator gave a residual error of 1.7e-5 against
 // the fp64 oracle, above the 1e-5 bar.
 //
-// A CTA of two warpgroups owns a tile of 64 jet rows (TP = 64 / C points x C channels, row r = c TP + pl); both
-// warpgroups issue wgmma.mma_async m64n64k8 over all 64 rows (N / 64 column blocks, and one m64n32k8 block when N is an
-// odd multiple of 32): warpgroup 0 accumulates
-// A_hi B_hi, warpgroup 1 A_lo B_hi + A_hi B_lo, both in registers; the epilogue adds the two through shared memory.  Per
-// 32-wide K chunk all threads write the activation jets of the previous layer's pre-activations, split into hi / lo,
-// into the chunk's A stage (K-major, 128-byte rows, 128-byte swizzle); one thread stages the chunk of the pre-swizzled
-// weight image (prepared once per call by k_wg_prep_w) with a TMA bulk copy onto an mbarrier.  Two stages: the MMAs of
-// chunk j run while the operands of chunk j + 1 are produced.  Persistent: CTA b handles tiles b, b + grid, ...
+// A CTA of two warpgroups owns a tile of 64 jet rows (TP = 64 / C points x C channels, row r = c TP + pl) and all N
+// output columns.  Warpgroup w owns columns [w N / 2, (w + 1) N / 2) with both accumulators in registers and issues, per
+// K step of 8, three wgmma.mma_async m64n(N/2)k8 over all 64 rows:  A_hi B_hi -> exact,  A_lo B_hi -> cross,
+// A_hi B_lo -> cross (the sequence of k_wg_dw).  The two warpgroups run one instruction stream and differ only in the row
+// offset of their B descriptors; A is read from shared memory once per term.  Per 32-wide K chunk all threads write the
+// activation jets of the previous layer's pre-activations, split into hi / lo, into the chunk's A stage (K-major,
+// 128-byte rows, 128-byte swizzle); one thread stages the chunk of the pre-swizzled weight image (prepared once per
+// call by k_wg_prep_w) with a TMA bulk copy onto an mbarrier.  Two stages: the MMAs of chunk j run while the operands of
+// chunk j + 1 are produced, and the global loads of chunk j + 2's A operand (across tile boundaries too) are in flight
+// in registers.  The epilogue forms exact + cross in registers; both warpgroups write their column halves.
+// Persistent: CTA b handles tiles b, b + grid, ...
 #pragma once
 
 #include "kernels_thin.cuh"
@@ -35,8 +38,10 @@ constexpr int A_TILE_BYTES = TM * KCH * 4;   // 8 KB (one of hi / lo)
 __host__ __device__ inline int tile_points(int C) { return TM / C; }
 
 __host__ __device__ inline int stage_bytes(int N) { return 2 * A_TILE_BYTES + 2 * N * KCH * 4; }
-// two stages, then an all-zero A tile (operand of warpgroup 0's second MMA per K step), then the mbarriers
-__host__ __device__ inline int fwd_smem_bytes(int N) { return 2 * stage_bytes(N) + A_TILE_BYTES + 1024 + 64; }
+// two stages, then the mbarriers
+__host__ __device__ inline int fwd_smem_bytes(int N) { return 2 * stage_bytes(N) + 1024 + 64; }
+// k_wg_layer keeps the next chunk's A-operand loads in registers for jet layouts of up to this many channels
+constexpr int PREFETCH_MAX_CS = 8;
 
 // byte offset of element (row, kk) inside a [rows x 32 fp32] K-major 128-byte-swizzled tile
 __host__ __device__ __forceinline__ uint32_t sw128(int row, int kk) {
@@ -103,34 +108,44 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// D[64 x 64] (+)= A[64 x 8] B[8 x 64], tf32 operands from shared memory, fp32 accumulators in registers
-__device__ __forceinline__ void wgmma_tf32_m64n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "%32, %33, p, 1, 1;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
-        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
-        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(accumulate));
-}
-
-// D[64 x 32] (+)= A[64 x 8] B[8 x 32]
-__device__ __forceinline__ void wgmma_tf32_m64n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "%16, %17, p, 1, 1;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "r"(accumulate));
-}
+// D[64 x M] (+)= A[64 x 8] B[8 x M], M = 16, 32, .. 128: tf32 operands from shared memory, fp32 accumulators in
+// registers (M / 2 per thread: the fragments of the M / 8 n8 blocks one after the other).  WG_Tg / WG_Og: registers
+// 0 .. 8 g + 7 in the instruction text and as operands; IA, IB, IP: the numbers of the operands that follow them.
+#define WG_T0 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define WG_T1 WG_T0 ", %8, %9, %10, %11, %12, %13, %14, %15"
+#define WG_T2 WG_T1 ", %16, %17, %18, %19, %20, %21, %22, %23"
+#define WG_T3 WG_T2 ", %24, %25, %26, %27, %28, %29, %30, %31"
+#define WG_T4 WG_T3 ", %32, %33, %34, %35, %36, %37, %38, %39"
+#define WG_T5 WG_T4 ", %40, %41, %42, %43, %44, %45, %46, %47"
+#define WG_T6 WG_T5 ", %48, %49, %50, %51, %52, %53, %54, %55"
+#define WG_T7 WG_T6 ", %56, %57, %58, %59, %60, %61, %62, %63"
+#define WG_O8(b) "+f"(d[b]), "+f"(d[b + 1]), "+f"(d[b + 2]), "+f"(d[b + 3]), "+f"(d[b + 4]), "+f"(d[b + 5]), "+f"(d[b + 6]), "+f"(d[b + 7])
+#define WG_O0 WG_O8(0)
+#define WG_O1 WG_O0, WG_O8(8)
+#define WG_O2 WG_O1, WG_O8(16)
+#define WG_O3 WG_O2, WG_O8(24)
+#define WG_O4 WG_O3, WG_O8(32)
+#define WG_O5 WG_O4, WG_O8(40)
+#define WG_O6 WG_O5, WG_O8(48)
+#define WG_O7 WG_O6, WG_O8(56)
+#define WG_MMA(M, G, IA, IB, IP)                                                                                  \
+  __device__ __forceinline__ void wgmma_tf32(float (&d)[M / 2], uint64_t da, uint64_t db, uint32_t accumulate) { \
+    asm volatile(                                                                                                 \
+        "{\n\t.reg .pred p;\n\t"                                                                                  \
+        "setp.ne.b32 p, %" #IP ", 0;\n\t"                                                                          \
+        "wgmma.mma_async.sync.aligned.m64n" #M "k8.f32.tf32.tf32 {" WG_T##G "}, %" #IA ", %" #IB ", p, 1, 1;\n\t}"  \
+        : WG_O##G                                                                                                 \
+        : "l"(da), "l"(db), "r"(accumulate));                                                                     \
+  }
+WG_MMA(16, 0, 8, 9, 10)
+WG_MMA(32, 1, 16, 17, 18)
+WG_MMA(48, 2, 24, 25, 26)
+WG_MMA(64, 3, 32, 33, 34)
+WG_MMA(80, 4, 40, 41, 42)
+WG_MMA(96, 5, 48, 49, 50)
+WG_MMA(112, 6, 56, 57, 58)
+WG_MMA(128, 7, 64, 65, 66)
+#undef WG_MMA
 
 // ---- weight image: img[j][part][sw128(n, kk)] = split(B[n][32 j + kk]), part 0 = hi, 1 = lo ----------------------
 // transposed = 0: B[n][k] = W[k N + n]   (forward: W is [K = in][N = out] row-major)
@@ -166,8 +181,8 @@ struct WgArgs {
   int act;
 };
 
-// Epilogue scratch, free once every MMA of the tile has retired: the B region of stage 0 takes warpgroup 1's accumulators
-// (fragment order), the B region of stage 1 the dx exchange tile [64 rows][N] (16-byte chunks XOR-swizzled by r & 7).
+// dx epilogue scratch, free once every MMA of the tile has retired: the B region of stage 1 takes the exchange tile
+// [64 rows][N] (16-byte chunks XOR-swizzled by r & 7).
 __device__ __forceinline__ unsigned char* xchg(unsigned char* base_ptr, int sbytes, int N, int r, int col) {
   return base_ptr + sbytes + 2 * A_TILE_BYTES + r * N * 4 + ((((col >> 2) ^ r) & 7) << 4) + (((col >> 2) & ~7) << 4) +
          (col & 3) * 4;
@@ -186,10 +201,12 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_layer(WgArgs g) {
   constexpr int rows_used = CS * TP;
   constexpr int PPR = (THREADS / 32) * 4;  // points per pass of the producers
   constexpr int MAXI = (TP + PPR - 1) / PPR;
-  constexpr int N = NQ * 32;  // output columns: NB blocks of 64, then a block of 32 if TAIL
-  constexpr int NB = NQ / 2, TAIL = NQ & 1;
+  constexpr int N = NQ * 32;  // output columns
+  constexpr int NH = N / 2;   // ... of one warpgroup: one m64nNHk8 per term and K step
+  // the A operand's global loads run one chunk ahead in MAXI CS float4 registers per thread
+  constexpr bool PREFETCH = CS <= PREFETCH_MAX_CS;
   const int sbytes = stage_bytes(N);
-  const uint32_t bar0 = base + 2 * sbytes + A_TILE_BYTES;  // two mbarriers: weight chunk of stage 0 / 1 landed
+  const uint32_t bar0 = base + 2 * sbytes;  // two mbarriers: weight chunk of stage 0 / 1 landed
   const uint32_t b_bytes = (uint32_t)(2 * N * KCH * 4);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wgi = tid >> 7;
   const int kq = lane & 7, psub = lane >> 3;
@@ -201,23 +218,42 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_layer(WgArgs g) {
     mbar_init(bar0 + 8, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  for (int s = 0; s < 3; ++s) {  // A pad rows (>= rows_used) stay zero operands for good; s = 2: the zero tile
+  for (int s = 0; s < 2; ++s) {  // A pad rows (>= rows_used) stay zero operands for good
     float4* az = reinterpret_cast<float4*>(base_ptr + s * sbytes);
-    for (int i = tid; i < (s < 2 ? 2 : 1) * A_TILE_BYTES / 16; i += THREADS) az[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i = tid; i < 2 * A_TILE_BYTES / 16; i += THREADS) az[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
   fence_proxy_async();
   __syncthreads();
 
-  float acc[NB > 0 ? NB : 1][32], acct[TAIL ? 16 : 1];
-  // registers of accumulator fragment (row group h, columns 8 j + 2 (lane & 3) + b): element 2 h + b of n8 block j
-  auto frag = [&](int j, int i) -> float& { return j < 8 * NB ? acc[j >> 3][4 * (j & 7) + i] : acct[4 * (j - 8 * NB) + i]; };
+  // A operand: item = (point, 4 consecutive k); a quarter warp holds the 8 items of one point's chunk.  z: the
+  // pre-activation jets (dx: the plain operand) of this thread's items of one chunk; zok: the item exists
+  float4 z[MAXI][CS];
+  bool zok[MAXI];
+  auto load_z = [&](int tile, int j) {
+#pragma unroll
+    for (int i = 0; i < MAXI; ++i) {
+      const int pl = warp * 4 + psub + i * PPR;
+      const long long p = (long long)tile * TP + pl;
+      zok[i] = pl < TP && tile < g.num_tiles && p < g.Np;
+      if (g.Kvalid && j * KCH + 4 * kq >= g.Kvalid) zok[i] = false;  // zero columns beyond a padded contraction length
+      const float* src = g.A.Z + p * g.A.ld + j * KCH + 4 * kq;
+#pragma unroll
+      for (int c = 0; c < CS; ++c)
+        z[i][c] = zok[i] ? __ldg(reinterpret_cast<const float4*>(src + (long long)c * g.A.plane)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  };
+  if constexpr (PREFETCH) load_z(blockIdx.x, 0);
+
+  // accumulator fragments of this warpgroup's columns (exact term, cross terms): element 4 j + 2 h + b is row
+  // rbase + 8 h, column wgi NH + 8 j + 2 (lane & 3) + b
+  float ex[NH / 2], cr[NH / 2];
+  const int rbase = (warp & 3) * 16 + (lane >> 2);
+  const int cbase = wgi * NH + 2 * (lane & 3);
   uint32_t it = 0;  // running chunk counter: stage it & 1, use (it >> 1) of that stage
   for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
     const long long p0 = (long long)tile * TP;
 #pragma unroll
-    for (int j = 0; j < N / 8; ++j)
-#pragma unroll
-      for (int i = 0; i < 4; ++i) frag(j, i) = 0.f;
+    for (int e = 0; e < NH / 2; ++e) ex[e] = cr[e] = 0.f;
     for (int j = 0; j < nchunks; ++j, ++it) {
       const uint32_t s = it & 1u;
       wgmma_wait<1>();  // this warpgroup's MMAs of chunk it - 2 (the last reader of stage s) have retired
@@ -228,24 +264,18 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_layer(WgArgs g) {
         mbar_expect_tx(bar0 + 8 * s, b_bytes);
         bulk_g2s(st_addr + 2 * A_TILE_BYTES, g.Wimg + (long long)j * 2 * N * KCH, b_bytes, bar0 + 8 * s);
       }
-      // A operand of this chunk: item = (point, 4 consecutive k); a quarter warp writes the 8 chunks of one row
+      if constexpr (!PREFETCH) load_z(tile, j);
+      // A operand of this chunk: a quarter warp writes the 8 16-byte chunks of one row
 #pragma unroll
       for (int i = 0; i < MAXI; ++i) {
         const int pl = warp * 4 + psub + i * PPR;
         if (pl >= TP) continue;
-        const long long p = p0 + pl;
-        bool valid = p < g.Np;
-        const float* src = g.A.Z + p * g.A.ld + j * KCH + 4 * kq;
-        if (g.Kvalid && j * KCH + 4 * kq >= g.Kvalid) valid = false;  // zero columns beyond a padded contraction length
-        float4 z[CS];
-#pragma unroll
-        for (int c = 0; c < CS; ++c)
-          z[c] = valid ? __ldg(reinterpret_cast<const float4*>(src + (long long)c * g.A.plane)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const bool valid = zok[i];
         float yout[CS][4];
         if constexpr (DX) {  // plain operand
 #pragma unroll
           for (int c = 0; c < CS; ++c) {
-            yout[c][0] = z[c].x; yout[c][1] = z[c].y; yout[c][2] = z[c].z; yout[c][3] = z[c].w;
+            yout[c][0] = z[i][c].x; yout[c][1] = z[i][c].y; yout[c][2] = z[i][c].z; yout[c][3] = z[i][c].w;
           }
         } else {
 #pragma unroll
@@ -253,9 +283,9 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_layer(WgArgs g) {
             auto comp = [&](const float4& v) { return t == 0 ? v.x : t == 1 ? v.y : t == 2 ? v.z : v.w; };
             float sc[6];
             float y0;
-            act_coef<float, L::KM>(act, comp(z[0]), y0, sc);
+            act_coef<float, L::KM>(act, comp(z[i][0]), y0, sc);
             yout[0][t] = valid ? y0 : 0.f;
-            jet_fwd<float, L>(g.J, sc, [&](int c) { return comp(z[c]); }, [&](int c, float v) { yout[c][t] = valid ? v : 0.f; });
+            jet_fwd<float, L>(g.J, sc, [&](int c) { return comp(z[i][c]); }, [&](int c, float v) { yout[c][t] = valid ? v : 0.f; });
           }
         }
 #pragma unroll
@@ -268,68 +298,42 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_layer(WgArgs g) {
           *reinterpret_cast<float4*>(st_ptr + A_TILE_BYTES + off) = l;
         }
       }
+      if constexpr (PREFETCH) {  // the next chunk's loads land while this chunk's MMAs are issued and the older ones run
+        if (j + 1 < nchunks) load_z(tile, j + 1);
+        else load_z(tile + gridDim.x, 0);
+      }
       fence_proxy_async();
       __syncthreads();
       mbar_wait(bar0 + 8 * s, (it >> 1) & 1u);
-      // MMAs of this chunk: warpgroup 0 the exact-product term, warpgroup 1 the two cross terms
+      // MMAs of this chunk.  Both warpgroups issue the same instruction sequence (the compiler serialises wgmma issued on
+      // divergent paths); warpgroup 1's B rows start N / 2 rows (a multiple of the 8-row swizzle group) further on
       const uint64_t a_hi = make_desc(st_addr), a_lo = make_desc(st_addr + A_TILE_BYTES);
-      const uint64_t b_hi = make_desc(st_addr + 2 * A_TILE_BYTES), b_lo = make_desc(st_addr + 2 * A_TILE_BYTES + N * 128);
-      // Both warpgroups issue the same instruction sequence (the compiler serialises wgmma issued on divergent paths):
-      // warpgroup 0 A_hi B_hi + 0 B_lo (the zero tile adds an exact 0), warpgroup 1 A_lo B_hi + A_hi B_lo
-      const uint64_t a1 = wgi ? a_lo : a_hi, a2 = wgi ? a_hi : make_desc(base + 2 * sbytes);
+      const uint64_t b_hi = make_desc(st_addr + 2 * A_TILE_BYTES + wgi * NH * 128), b_lo = b_hi + (uint64_t)(N * 128 / 16);
       wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < KCH / 8; ++ks) {
         const uint64_t inc = (uint64_t)(2 * ks);  // 32 bytes in units of 16
         const uint32_t first = (j == 0 && ks == 0) ? 0u : 1u;
-#pragma unroll
-        for (int nb = 0; nb < NB; ++nb) {
-          const uint64_t bo = inc + (uint64_t)(nb * 64 * 128 / 16);  // column block nb = B rows 64 nb ..
-          wgmma_tf32_m64n64(acc[nb], a1 + inc, b_hi + bo, first);
-          wgmma_tf32_m64n64(acc[nb], a2 + inc, b_lo + bo, 1u);
-        }
-        if constexpr (TAIL) {
-          const uint64_t bo = inc + (uint64_t)(NB * 64 * 128 / 16);  // the last 32 columns
-          wgmma_tf32_m64n32(acct, a1 + inc, b_hi + bo, first);
-          wgmma_tf32_m64n32(acct, a2 + inc, b_lo + bo, 1u);
-        }
+        wgmma_tf32(ex, a_hi + inc, b_hi + inc, first);
+        wgmma_tf32(cr, a_lo + inc, b_hi + inc, first);
+        wgmma_tf32(cr, a_hi + inc, b_lo + inc, 1u);
       }
       wgmma_commit();
     }
     wgmma_wait<0>();
-    __syncthreads();  // every MMA of the tile has retired in both warpgroups: the B regions are free
-    {  // warpgroup 0 adds warpgroup 1's accumulators (fragment order, conflict-free)
-      float* xs = reinterpret_cast<float*>(base_ptr + 2 * A_TILE_BYTES);
-      const int lt = tid & 127;
-      if (wgi == 1) {
-#pragma unroll
-        for (int j = 0; j < N / 8; ++j)
-#pragma unroll
-          for (int i = 0; i < 4; ++i) xs[(4 * j + i) * 128 + lt] = frag(j, i);
-      }
-      __syncthreads();
-      if (wgi == 0) {
-#pragma unroll
-        for (int j = 0; j < N / 8; ++j)
-#pragma unroll
-          for (int i = 0; i < 4; ++i) frag(j, i) += xs[(4 * j + i) * 128 + lt];
-      }
-    }
-    const int rbase = (warp & 3) * 16 + (lane >> 2);  // warpgroup 0: accumulator rows rbase, rbase + 8 of this thread
     if constexpr (!DX) {
-      // ---- forward epilogue: accumulator fragments (+ bias) -> Z_l; row r = c TP + pl of the tile ----
+      // ---- forward epilogue: exact + cross (+ bias) -> Z_l; row r = c TP + pl of the tile ----
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = rbase + 8 * h;
-        if (wgi != 0) break;
         const int c = r / TP, pl = r - c * TP;
         const long long p = p0 + pl;
         if (r >= rows_used || p >= g.Np) continue;
         float* out_row = g.Out + (long long)c * g.oplane + p * g.ldo;
 #pragma unroll
-        for (int j = 0; j < N / 8; ++j) {
-          const int col = j * 8 + 2 * (lane & 3);
-          float2 v = make_float2(frag(j, 2 * h), frag(j, 2 * h + 1));
+        for (int j = 0; j < NH / 8; ++j) {
+          const int col = cbase + 8 * j;
+          float2 v = make_float2(ex[4 * j + 2 * h] + cr[4 * j + 2 * h], ex[4 * j + 2 * h + 1] + cr[4 * j + 2 * h + 1]);
           if (c == 0 && g.bias) {
             v.x += __ldg(g.bias + col);
             v.y += __ldg(g.bias + col + 1);
@@ -337,31 +341,46 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_layer(WgArgs g) {
           *reinterpret_cast<float2*>(out_row + col) = v;
         }
       }
-      fence_proxy_async();  // warpgroup 1's scratch writes are ordered before the next tile's bulk copies
     } else {
       // ---- dx epilogue: Abar (registers) -> exchange tile -> activation adjoint with Z_{l-1} -> Zbar_{l-1} ----
+      __syncthreads();  // every MMA of the tile has retired in both warpgroups: the B regions are free
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = rbase + 8 * h;
-        if (wgi != 0) break;
 #pragma unroll
-        for (int j = 0; j < N / 8; ++j) {
-          const int col = j * 8 + 2 * (lane & 3);
-          *reinterpret_cast<float2*>(xchg(base_ptr, sbytes, N, r, col)) = make_float2(frag(j, 2 * h), frag(j, 2 * h + 1));
-        }
+        for (int j = 0; j < NH / 8; ++j)
+          *reinterpret_cast<float2*>(xchg(base_ptr, sbytes, N, r, cbase + 8 * j)) =
+              make_float2(ex[4 * j + 2 * h] + cr[4 * j + 2 * h], ex[4 * j + 2 * h + 1] + cr[4 * j + 2 * h + 1]);
       }
-      __syncthreads();
+      // item = (point, 4 consecutive columns).  With PREFETCH the Z_{l-1} loads run one item ahead, those of the first
+      // item across the barrier
       constexpr int N4 = N / 4;
-      for (int item = tid; item < TP * N4; item += THREADS) {  // item = (point, 4 consecutive columns)
+      auto load_zc = [&](int item, float4 (&zc)[CS]) {
         const int pl = item / N4, q = item - pl * N4;
         const long long p = p0 + pl;
-        if (p >= g.Np) continue;
-        float4 zc[CS], xc[CS];
+        if (item >= TP * N4 || p >= g.Np) return;
 #pragma unroll
-        for (int c = 0; c < CS; ++c) {
+        for (int c = 0; c < CS; ++c)
           zc[c] = __ldg(reinterpret_cast<const float4*>(g.Zprev + (long long)c * g.zplane + p * g.ldz + 4 * q));
-          xc[c] = *reinterpret_cast<const float4*>(xchg(base_ptr, sbytes, N, c * TP + pl, 4 * q));
+      };
+      float4 znext[CS];
+      if constexpr (PREFETCH) load_zc(tid, znext);
+      __syncthreads();
+      for (int item = tid; item < TP * N4; item += THREADS) {
+        const int pl = item / N4, q = item - pl * N4;
+        const long long p = p0 + pl;
+        float4 zc[CS];
+        if constexpr (PREFETCH) {
+#pragma unroll
+          for (int c = 0; c < CS; ++c) zc[c] = znext[c];
+          load_zc(item + THREADS, znext);
+        } else {
+          load_zc(item, zc);
         }
+        if (p >= g.Np) continue;
+        float4 xc[CS];
+#pragma unroll
+        for (int c = 0; c < CS; ++c) xc[c] = *reinterpret_cast<const float4*>(xchg(base_ptr, sbytes, N, c * TP + pl, 4 * q));
         float ob[CS][4];
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
@@ -377,7 +396,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_layer(WgArgs g) {
         for (int c = 0; c < CS; ++c)
           *reinterpret_cast<float4*>(out + (long long)c * g.oplane) = make_float4(ob[c][0], ob[c][1], ob[c][2], ob[c][3]);
       }
-      fence_proxy_async();  // the exchange writes are ordered before the next tile's bulk copies into the B regions
+      fence_proxy_async();  // the exchange tile's accesses are ordered before the next tile's bulk copies into the B regions
       __syncthreads();
     }
   }
