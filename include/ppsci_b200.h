@@ -172,6 +172,15 @@ typedef struct ppsci_plan_spec {
    * gradient buffers: [W_1 | b_1 | ... | W_L | b_L | Wu | bu | Wv | bv | alpha_0 ... alpha_{B-1}].  Gated plans run on
    * the CUDA-core kernels (csrc/kernels_gate.cuh + the generic tile GEMMs); two-phase value calls are not offered. */
   int32_t gated;
+  /* Trainable PeriodEmbedding frequencies (ppsci/arch/mlp.py:95-114, ParamAttr(trainable=True)): n_omega scalars
+   * omega_0 .. omega_{n_omega-1} at the END of the parameter / gradient buffers, behind everything else:
+   *   [... | betas | omega_0 ... omega_{n_omega-1}]
+   * Feature f (a cos / sin feature) with feat_omega_param[f] = j >= 0 reads omega_j from `params` on the device at every
+   * call (feat_omega[f] is then ignored), and every call that takes `grads` accumulates dLoss/d omega_j there (summed in
+   * fp64 within the call).  feat_omega_param[f] = -1: the fixed feat_omega[f].  n_omega = 0 ignores feat_omega_param, so
+   * a zero-filled tail builds the plan of fixed frequencies.  Not with dense_in. */
+  int32_t n_omega;
+  int32_t feat_omega_param[PPSCI_MAX_FEAT];
 } ppsci_plan_spec;
 
 typedef struct ppsci_plan ppsci_plan;
@@ -182,7 +191,8 @@ int ppsci_b200_plan_create(const ppsci_plan_spec* spec, ppsci_plan** out);
 void ppsci_b200_plan_destroy(ppsci_plan* plan);
 
 /* Number of parameters in the flat buffer: for each layer l, W_l [in,out] row-major
- * (the reference's nn.Linear layout, ppsci/arch/mlp.py:246,274) followed by b_l [out]. */
+ * (the reference's nn.Linear layout, ppsci/arch/mlp.py:246,274) followed by b_l [out]; then the gated networks'
+ * embeddings and alphas, the activations' betas and the n_omega trainable frequencies. */
 int64_t ppsci_b200_plan_param_count(const ppsci_plan* plan);
 
 /* Where the loss-and-gradient calls ACCUMULATE dLoss/d(aux parameter `aux_index`) (a device fp64 scalar owned by the

@@ -173,9 +173,15 @@ class MLP(base.Arch):
     (FourierEmbedding, mlp.py:117-136, applied after the period embedding, mlp.py:298-315) is one more linear layer
     for the kernels: ``[cos(x B), sin(x B)] = sin(x [B | B] + [pi/2 | 0])`` — tied effective weights, a constant bias
     and ``sin`` as that layer's activation (``NetSpec.act_first``); the gradient of the trainable kernel ``B`` is the
-    sum of the two halves of the effective layer's weight gradient.  Not yet supported (raise ``NotImplementedError``
-    at construction): trainable periods.  ``fourier`` composes with weight_norm / random_weight / skip_connection (one
-    staging buffer: the tied first layer in front of the reparametrised linear layers).
+    sum of the two halves of the effective layer's weight gradient.  ``fourier`` composes with weight_norm / random_weight /
+    skip_connection (one staging buffer: the tied first layer in front of the reparametrised linear layers).
+
+    ``periods={key: (period, trainable)}`` (PeriodEmbedding, mlp.py:95-114): the features ``[cos(w x), sin(w x)]`` with
+    ``w = 2 pi / period``.  A trainable key's ``w`` is a parameter: one scalar per trainable key, in the order of the
+    ``periods`` dict, at the END of ``flat`` (behind the Fourier kernel; with ``grad_clip`` it falls in the trailing
+    segment with the gains / alphas / betas / kernel) and at the end of the buffer the kernels read, which read it on the
+    device at every call and accumulate dLoss/dw beside the weight gradient.  Checkpoint key: ``period_emb.freqs.{i}``, i
+    the key's position in ``periods`` (fixed keys emit none).
     """
 
     # 1: ModifiedMLP (two embedding layers + the gate after every hidden layer); 2: PirateNet (blocks of three layers,
@@ -227,19 +233,23 @@ class MLP(base.Arch):
         feat_src: List[int] = []
         feat_kind: List[int] = []
         feat_omega: List[float] = []
+        feat_omega_param: List[int] = []
+        # trainable frequencies: (position of the key in ``periods``, key), the order of their entries in ``flat``
+        self._omega_keys = [(i, k) for i, (k, (_, tr)) in enumerate((self.periods or {}).items()) if tr]
+        omega_index = {k: j for j, (_, k) in enumerate(self._omega_keys)}
         for i, k in enumerate(self.input_keys):
             if self.periods and k in self.periods:
                 p, trainable = self.periods[k]
-                if trainable:
-                    raise NotImplementedError("trainable periods are not supported by the jet kernels yet")
                 w = 2 * np.pi / float(p)
                 feat_src += [i, i]
                 feat_kind += [1, 2]
                 feat_omega += [w, w]
+                feat_omega_param += [omega_index.get(k, -1)] * 2
             else:
                 feat_src.append(i)
                 feat_kind.append(0)
                 feat_omega.append(0.0)
+                feat_omega_param.append(-1)
         if self.periods:
             for k in self.periods:
                 if k not in self.input_keys:
@@ -255,9 +265,11 @@ class MLP(base.Arch):
         if self._beta_len and self._gated:
             raise NotImplementedError(f"{type(self).__name__}(activation={self.activation!r}): activations with a trainable "
                                       "parameter are supported by the plain MLP plans only")
+        n_omega = len(self._omega_keys)
         self._net = NetSpec(self.input_keys, self.output_keys, feat_src, feat_kind, feat_omega, eng_widths,
                             {"swish": "swish_b"}.get(self.activation, self.activation),
-                            act_first="sin" if self.fourier else None, gated=int(self._gated))
+                            act_first="sin" if self.fourier else None, gated=int(self._gated),
+                            feat_omega_param=feat_omega_param if n_omega else None, n_omega=n_omega)
         self._shapes = list(zip(widths[:-1], widths[1:]))
         self._n_hidden = len(hidden)
         if self._gated:  # embed_u / embed_v (n_feat -> hidden[0]) stored behind last_fc: [... | Wu | bu | Wv | bv]
@@ -288,6 +300,8 @@ class MLP(base.Arch):
             self._f_off = off
             off += nf * dh
             self._f_n0 = nf * 2 * dh + 2 * dh
+        self._omega_off, self._n_omega = off, n_omega  # trainable frequencies: the last entries of flat
+        off += n_omega
         self.flat = nn.Parameter(torch.zeros(off, dtype=dtype))
         self.linears = [_LinearView(self, i) for i in range(len(hidden))]
         self.last_fc = _LinearView(self, len(hidden))
@@ -304,11 +318,12 @@ class MLP(base.Arch):
         self.skip_connection = bool(skip_connection)
         self._skip_layers = [i for i in range(len(hidden)) if self.skip_connection and i % 2 == 0 and i >= 2]
         self._reparam = Reparam(self._shapes, 0, self._n_eff, self._g_off, self.weight_norm, self._skip_slices())
-        # the engine reads effective weights from a staging buffer [W0 | b0 (fourier) | reparametrised linear layers]
+        # the engine reads effective weights from a staging buffer [W0 | b0 (fourier) | reparametrised linear layers | w]
         self._has_eff = bool(self.weight_norm or self.random_weight or self.fourier or self._skip_layers)
         if self._has_eff:
-            self.register_buffer("_eff", torch.zeros(self._f_n0 + self._n_eff, dtype=dtype), persistent=False)
-            self.register_buffer("_eff_grad", torch.zeros(self._f_n0 + self._n_eff, dtype=dtype), persistent=False)
+            n_stage = self._f_n0 + self._n_eff + n_omega
+            self.register_buffer("_eff", torch.zeros(n_stage, dtype=dtype), persistent=False)
+            self.register_buffer("_eff_grad", torch.zeros(n_stage, dtype=dtype), persistent=False)
         self.reset_parameters()
         self._value_plan = None
 
@@ -341,6 +356,13 @@ class MLP(base.Arch):
                 nf, dh = self._f_shape
                 k = torch.randn(nf * dh, dtype=torch.float64) * float(self.fourier["scale"])
                 self.flat.data[self._f_off: self._f_off + nf * dh] = k.to(self.flat.dtype)
+            for j, (_, k) in enumerate(self._omega_keys):  # Constant(2 pi / period) (mlp.py:97-104)
+                self.flat.data[self._omega_off + j] = 2 * np.pi / float(self.periods[k][0])
+
+    @property
+    def period_freqs(self) -> torch.Tensor:
+        """View of the trainable frequencies [n_trainable] (``period_emb.freqs`` of the trainable keys)."""
+        return self.flat.data[self._omega_off: self._omega_off + self._n_omega]
 
     @property
     def fourier_kernel(self) -> torch.Tensor:
@@ -377,7 +399,9 @@ class MLP(base.Arch):
         if not self._has_eff:
             return self.flat.data
         with torch.no_grad():
-            self._reparam.fill(self.flat.data, self._eff[self._f_n0:])
+            n_lin = self._f_n0 + self._n_eff
+            self._reparam.fill(self.flat.data, self._eff[self._f_n0: n_lin])
+            self._eff[n_lin:].copy_(self.flat.data[self._omega_off:])
             if self.fourier:
                 nf, dh = self._f_shape
                 k = self.fourier_kernel
@@ -403,7 +427,9 @@ class MLP(base.Arch):
             return
         with torch.no_grad():
             gr = self.flat.grad
-            self._reparam.chain(self.flat.data, gr, self._eff_grad[self._f_n0:])
+            n_lin = self._f_n0 + self._n_eff
+            self._reparam.chain(self.flat.data, gr, self._eff_grad[self._f_n0: n_lin])
+            gr[self._omega_off:] += self._eff_grad[n_lin:]
             if self.fourier:  # the tied kernel takes the sum of both halves; the constant bias [pi/2 | 0] takes none
                 nf, dh = self._f_shape
                 dw0 = self._eff_grad[: nf * 2 * dh].view(nf, 2 * dh)
@@ -438,13 +464,23 @@ class MLP(base.Arch):
             out[f"acts.{i}.beta"] = b if self.activation == "stan" else b.reshape(())
         if self.fourier:
             out["fourier_emb.kernel"] = self.fourier_kernel.detach().clone()
+        for j, (i, _) in enumerate(self._omega_keys):  # nn.ParameterList of 0-d parameters (mlp.py:97-105)
+            out[f"period_emb.freqs.{i}"] = self.period_freqs[j].detach().clone()
         return out
 
     def load_state_dict(self, state_dict, strict: bool = True):
         views = self._views()
         known = self._layer_names() + (["fourier_emb"] if self.fourier else []) + [f"acts.{i}" for i in range(len(self._beta_off))]
-        missing, unexpected = [], [k for k in state_dict if k.rsplit(".", 1)[0] not in known]
+        freq_keys = [f"period_emb.freqs.{i}" for i, _ in self._omega_keys]
+        missing, unexpected = [], [k for k in state_dict if k.rsplit(".", 1)[0] not in known and k not in freq_keys]
         with torch.no_grad():
+            for j, key in enumerate(freq_keys):
+                if key not in state_dict:
+                    missing.append(key)
+                    continue
+                src = state_dict[key]
+                src = torch.as_tensor(np.asarray(src.cpu() if hasattr(src, "cpu") else src)).reshape(-1)
+                self.period_freqs[j: j + 1].copy_(src.to(self.flat.dtype).to(self.flat.device))
             for i, (o, n_b) in enumerate(zip(self._beta_off, self._beta_len)):
                 key = f"acts.{i}.beta"
                 if key not in state_dict:

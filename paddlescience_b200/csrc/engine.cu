@@ -60,6 +60,7 @@ struct ppsci_plan {
   // layer l, behind everything else; actp_stride 1 / 0, actp_off[l] < 0: layer l's activation has none
   int64_t actp_off[PPSCI_MAX_LAYERS + 1];
   int actp_stride = 0;
+  int64_t omega_off = 0;  // spec.n_omega trainable frequencies, the last entries of the buffers
   int ld_hidden_max = 4;
   int chunk = 0;
   int num_sms = 132;
@@ -133,6 +134,7 @@ struct Carve {
   size_t gt[PPSCI_MAX_LAYERS + 1];
   size_t zu, zv, zub, zvb;
   size_t xres, wtu, wtv;  // gated == 2: adjoint carried by the blocks' residual path; transposed embedding weights
+  size_t omega_acc;       // fp64 dLoss/d omega accumulators of a call (n_omega)
   size_t total;
 };
 
@@ -172,6 +174,7 @@ static void carve(const ppsci_plan* P, int64_t nc, Carve* cv) {
   cv->xres = take(pirate ? (size_t)P->C * nc * P->ld[1] * es : 0);
   cv->wtu = take(gated && emb ? (size_t)P->spec.widths[1] * P->spec.widths[lg] * es : 0);
   cv->wtv = take(gated && emb ? (size_t)P->spec.widths[1] * P->spec.widths[lg] * es : 0);
+  cv->omega_acc = take((size_t)P->spec.n_omega * sizeof(double));
   cv->total = off;
 }
 
@@ -282,6 +285,13 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
       return fail("plan_create: pgrad_aux must name a learnable (aux_bcast) parameter");
     if (s->pgrad_reg[g] < 0 || s->pgrad_reg[g] >= s->n_reg) return fail("plan_create: pgrad_reg out of range");
   }
+  if (s->n_omega < 0 || s->n_omega > PPSCI_MAX_FEAT) return fail("plan_create: n_omega out of range");
+  if (s->n_omega > 0 && s->dense_in) return fail("plan_create: dense_in plans take no trainable frequencies");
+  for (int f = 0; f < (s->n_omega > 0 ? s->n_feat : 0); ++f) {
+    const int j = s->feat_omega_param[f];
+    if (j < -1 || j >= s->n_omega) return fail("plan_create: feat_omega_param out of range");
+    if (j >= 0 && s->feat_kind[f] == PPSCI_FEAT_ID) return fail("plan_create: only cos / sin features take a trainable frequency");
+  }
 
   ppsci_plan* P = new ppsci_plan();
   P->spec = *s;
@@ -333,6 +343,8 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
     P->actp_off[l] = off;
     off += a_l == PPSCI_ACT_STAN ? s->widths[l] : 1;
   }
+  P->omega_off = off;
+  off += s->n_omega;
   P->n_params = off;
   // default points per workspace chunk: large chunks amortise kernel prologues / tails and give the dW kernels long
   // reductions per split (measured on cfg3: 65,536 -> 77.7 ms/step, 262,144 -> 73.7 ms/step); capped below by memory
@@ -485,7 +497,7 @@ extern "C" size_t ppsci_b200_plan_workspace_bytes(const ppsci_plan* P, int64_t n
 
 // ---------------------------------------------------------------------------------------------
 template <typename T>
-static void fill_seed(const ppsci_plan* P, const void* const* x_cols, int64_t x_off, AOperand<T>* A) {
+static void fill_seed(const ppsci_plan* P, const void* const* x_cols, int64_t x_off, const T* params, AOperand<T>* A) {
   const ppsci_plan_spec& s = P->spec;
   A->mode = A_SEED;
   A->act = s.act;
@@ -500,7 +512,9 @@ static void fill_seed(const ppsci_plan* P, const void* const* x_cols, int64_t x_
     S.feat_src[f] = f < s.n_feat ? s.feat_src[f] : 0;
     S.feat_kind[f] = f < s.n_feat ? s.feat_kind[f] : 0;
     S.feat_omega[f] = f < s.n_feat ? s.feat_omega[f] : 0.0;
+    S.omega_idx[f] = (s.n_omega > 0 && f < s.n_feat) ? s.feat_omega_param[f] : -1;
   }
+  S.omega = params + P->omega_off;
   for (int d = 0; d < PPSCI_MAX_DIR; ++d)
     for (int i = 0; i < PPSCI_MAX_IN; ++i) S.dir_vec[d][i] = (d < s.n_dir && i < s.n_in) ? s.dir_vec[d][i] : 0.0;
   for (int i = 0; i < PPSCI_MAX_IN; ++i) S.x_cols[i] = i < s.n_in ? x_cols[i] : nullptr;
@@ -519,12 +533,12 @@ static void fill_act(const ppsci_plan* P, const T* Z, int ld, int64_t nc, int mo
 
 // first-layer operand: input seeds, or (dense_in) the caller's row-major [n_points][n_feat] matrix as a plain operand
 template <typename T>
-static void fill_first(const ppsci_plan* P, const void* const* x_cols, int64_t x_off, int64_t nc, AOperand<T>* A) {
+static void fill_first(const ppsci_plan* P, const void* const* x_cols, int64_t x_off, int64_t nc, const T* params, AOperand<T>* A) {
   if (P->spec.dense_in) {
     const int nf = P->spec.n_feat;
     fill_act<T>(P, reinterpret_cast<const T*>(x_cols[0]) + x_off * nf, nf, nc, A_PLAIN, A);
   } else {
-    fill_seed<T>(P, x_cols, x_off, A);
+    fill_seed<T>(P, x_cols, x_off, params, A);
   }
 }
 
@@ -642,7 +656,7 @@ static int run(ppsci_plan* P, const CallArgs& a) {
     AOperand<T> A;
     memset(&A, 0, sizeof(A));
     if (l == 1) {
-      fill_first<T>(P, a.x_cols, c0, nc_max, &A);
+      fill_first<T>(P, a.x_cols, c0, nc_max, params, &A);
     } else if (gated) {
       fill_act<T>(P, reinterpret_cast<const T*>(ws + cv.gt[l - 1]), P->ld[l - 1], nc_max, A_PLAIN, &A);
     } else {
@@ -680,11 +694,15 @@ static int run(ppsci_plan* P, const CallArgs& a) {
 #endif
 
   if (a.want_loss) CK(cudaMemsetAsync(loss_acc, 0, PPSCI_MAX_RES * sizeof(double), st));
+  double* omega_acc = reinterpret_cast<double*>(ws + cv.omega_acc);
   // phase 1 runs the forward exactly as a training call would (stash of everything the adjoint reads), phase 2 only the adjoint
   const bool do_bwd = ((a.want_loss || a.ybar_in) && grads != nullptr) || a.phase == 1;
   if (a.phase == 2 && a.n_points > nc_max)
     return fail("values_bwd_kept: the kept stash covers one workspace chunk (" + std::to_string(nc_max) + " points); got " +
                 std::to_string(a.n_points));
+  // dLoss/d omega of the trainable frequencies: fp64 sums over the call, added to grads at its end
+  const bool omega_bwd = do_bwd && a.phase != 1 && s.n_omega > 0;
+  if (omega_bwd) CK(cudaMemsetAsync(omega_acc, 0, (size_t)s.n_omega * sizeof(double), st));
   if (do_bwd) {  // W_l^T for l >= 2; the embeddings hand an adjoint back to layer 1's output: Wu^T, Wv^T (layer 2's shape)
     struct Transpose {
       int l;       // layer whose shape the weights have
@@ -935,11 +953,15 @@ static int run(ppsci_plan* P, const CallArgs& a) {
         f.db = grads + P->b_off[1];
         f.Np = nc;
         f.pts_per_block = 32;
-        void (*k)(FirstArgs<T>) = k_first_dw<T, KMAX>;
+        f.W = params + P->w_off[1];
+        f.omega_grad = omega_acc;
+        void (*k)(FirstArgs<T>) = omega_bwd ? k_first_dw<T, KMAX, true> : k_first_dw<T, KMAX>;
         if constexpr (sizeof(T) == 4) {
           if (P->thin_vec && f.N % 4 == 0) {
             f.pts_per_block = 256;
-            with_lay(ThinLays{}, P->J, [&](auto lay) { k = thin::k_first_dw_v<decltype(lay)>; });
+            with_lay(ThinLays{}, P->J, [&](auto lay) {
+              k = omega_bwd ? thin::k_first_dw_v<decltype(lay), true> : thin::k_first_dw_v<decltype(lay)>;
+            });
           }
         }
         const dim3 grid((unsigned)((f.N + 255) / 256), (unsigned)((nc + f.pts_per_block - 1) / f.pts_per_block));
@@ -1012,6 +1034,30 @@ static int run(ppsci_plan* P, const CallArgs& a) {
             g.db = grads + P->gate_b_off[e];
             launch(CLS_DW, kw, grid_e, dim3(NTHREADS), smem_w, g);
           }
+        }
+        if (l == 1 && omega_bwd) {  // dLoss/d omega from every GEMM that read the seeds
+          OmegaArgs<T> o;
+          memset(&o, 0, sizeof(o));
+          o.A = operand(1, c0);
+          o.J = P->J;
+          o.nf = s.n_feat;
+          auto cons = [&](const T* zb, int lo, int64_t w_off) {
+            o.Zbar[o.n_cons] = zb;
+            o.ldzb[o.n_cons] = P->ld[lo];
+            o.zbplane[o.n_cons] = (long long)nc_max * P->ld[lo];
+            o.W[o.n_cons] = params + w_off;
+            o.N[o.n_cons] = s.widths[lo];
+            o.n_cons++;
+          };
+          cons(zbar(1), 1, P->w_off[1]);
+          if (gated && !emb) {  // ModifiedMLP without an embedding layer: embed_u / embed_v read the seeds too
+            cons(reinterpret_cast<const T*>(ws + cv.zub), 1, P->gate_w_off[0]);
+            cons(reinterpret_cast<const T*>(ws + cv.zvb), 1, P->gate_w_off[1]);
+          }
+          o.Np = nc;
+          o.omega_grad = omega_acc;
+          const long long want = (nc + 7) / 8, cap = 4LL * P->num_sms;
+          launch(CLS_MISC, k_omega_grad<T, KMAX>, dim3((unsigned)(want < cap ? want : cap)), dim3(256), 0, o);
         }
       }
       if (l == 1) break;
@@ -1096,6 +1142,9 @@ static int run(ppsci_plan* P, const CallArgs& a) {
       }
     }
   }
+  if (omega_bwd)
+    launch(CLS_MISC, k_omega_finish<T>, dim3((unsigned)((s.n_omega + 31) / 32)), dim3(32), 0, omega_acc, grads + P->omega_off,
+           (int)s.n_omega);
   if (a.want_loss && a.loss_out && s.n_res > 0)
     launch(CLS_MISC, k_finalize_loss<T>, dim3(1), dim3(32), 0, loss_acc, reinterpret_cast<T*>(a.loss_out), s.n_res);
   CK(cudaGetLastError());

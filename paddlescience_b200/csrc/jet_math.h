@@ -363,4 +363,34 @@ PPSCI_HD void seed_coef(int kind, T omega, T x, T v, T (&out)[5]) {
   }
 }
 
+// d/d omega of seed_coef's coefficients (a trainable PeriodEmbedding frequency; kind 1 / 2, identity features have none).
+// With G_k the k-th derivative of g at omega*x, the order-k coefficient G_k (omega v)^k / k! has the omega-derivative
+//   G_{k+1} x (omega v)^k / k!  +  G_k k omega^{k-1} v^k / k!        (value channel, k = 0:  G_1 x)
+template <typename T, int KMAX>
+PPSCI_HD void seed_dcoef(int kind, T omega, T x, T v, T (&out)[5]) {
+  if (kind == 0) {
+#if defined(__CUDACC__)
+#pragma unroll
+#endif
+    for (int k = 0; k <= KMAX; ++k) out[k] = T(0);
+    return;
+  }
+  T sn, cs;
+  m_sincos<T>(omega * x, &sn, &cs);
+  T g[6];
+  if (kind == 1) { g[0] = cs; g[1] = -sn; g[2] = -cs; g[3] = sn; g[4] = cs; g[5] = -sn; }
+  else           { g[0] = sn; g[1] = cs; g[2] = -sn; g[3] = -cs; g[4] = sn; g[5] = cs; }
+  const T h = omega * v;
+  const T inv_fact[5] = {T(1), T(1), T(0.5), T(1) / T(6), T(1) / T(24)};
+  T hp = T(1);  // h^(k-1)
+  out[0] = g[1] * x;
+#if defined(__CUDACC__)
+#pragma unroll
+#endif
+  for (int k = 1; k <= KMAX; ++k) {
+    out[k] = (g[k + 1] * x * hp * h + g[k] * T(k) * hp * v) * inv_fact[k];
+    hp *= h;
+  }
+}
+
 }  // namespace ppsci

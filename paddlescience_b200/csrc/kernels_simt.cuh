@@ -41,6 +41,10 @@ struct SeedSpec {
   double feat_omega[PPSCI_MAX_FEAT];
   double dir_vec[PPSCI_MAX_DIR][PPSCI_MAX_IN];
   const void* x_cols[PPSCI_MAX_IN];
+  // trainable frequencies (ppsci_plan_spec.feat_omega_param): feature f reads omega[omega_idx[f]] (of the plan's dtype,
+  // in the parameter buffer) at every call; omega_idx[f] < 0: the fixed feat_omega[f]
+  int omega_idx[PPSCI_MAX_FEAT];
+  const void* omega;
 };
 
 enum { A_SEED = 0, A_ACT = 1, A_PLAIN = 2 };
@@ -86,7 +90,7 @@ __device__ __forceinline__ void produce_a(const AOperand<T>& A, const JetLayout&
   const SeedSpec& S = A.seed;
   const int src = S.feat_src[k];
   const int kind = S.feat_kind[k];
-  const T omega = T(S.feat_omega[k]);
+  const T omega = S.omega_idx[k] >= 0 ? reinterpret_cast<const T*>(S.omega)[S.omega_idx[k]] : T(S.feat_omega[k]);
   const T x = reinterpret_cast<const T*>(S.x_cols[src])[A.x_off + p];
   T co[5];
   seed_coef<T, KMAX>(kind, omega, x, T(0), co);
@@ -98,6 +102,57 @@ __device__ __forceinline__ void produce_a(const AOperand<T>& A, const JetLayout&
 #pragma unroll
     for (int q = 0; q < KMAX; ++q)
       if (q < K) st(base + q, co[q + 1]);
+  }
+}
+
+// d/d omega of the C channels produce_a hands out for feature k of an A_SEED operand, k a trainable cos / sin feature
+// (seed.omega_idx[k] >= 0), at point p (< Np)
+template <typename T, int KMAX, typename St>
+__device__ __forceinline__ void produce_dseed(const AOperand<T>& A, const JetLayout& J, long long p, int k, St st) {
+  const SeedSpec& S = A.seed;
+  const int src = S.feat_src[k];
+  const int kind = S.feat_kind[k];
+  const T omega = reinterpret_cast<const T*>(S.omega)[S.omega_idx[k]];
+  const T x = reinterpret_cast<const T*>(S.x_cols[src])[A.x_off + p];
+  T co[5];
+  seed_dcoef<T, KMAX>(kind, omega, x, T(0), co);
+  st(0, co[0]);
+  for (int d = 0; d < J.n_dir; ++d) {
+    const int K = J.dir_order[d];
+    const int base = J.dir_base[d];
+    seed_dcoef<T, KMAX>(kind, omega, x, T(S.dir_vec[d][src]), co);
+#pragma unroll
+    for (int q = 0; q < KMAX; ++q)
+      if (q < K) st(base + q, co[q + 1]);
+  }
+}
+
+// dLoss/d omega: adds this CTA's shares part[f] of the features f < nf with omega_idx[f] >= 0 to out[omega_idx[f]] (fp64
+// accumulators in the workspace): summed in fp64 over the block, one atomic per CTA and frequency (the cos and sin
+// features of a period key share it).  Every thread of the block calls it; blockDim.x is a multiple of 32, at most 1024.
+template <typename T, int NF>
+__device__ void omega_flush(const T (&part)[NF], int nf, const int* omega_idx, double* out) {
+  __shared__ double red[NF][32];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  for (int f = 0; f < NF; ++f) {
+    if (f >= nf || omega_idx[f] < 0) continue;  // uniform across the block
+    double v = (double)part[f];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0) red[f][w] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  for (int f = 0; f < nf && f < NF; ++f) {
+    const int j = omega_idx[f];
+    bool first = j >= 0;
+    for (int e = 0; e < f && first; ++e) first = omega_idx[e] != j;
+    if (!first) continue;
+    double s = 0.0;
+    for (int e = f; e < nf && e < NF; ++e)
+      if (omega_idx[e] == j)
+        for (int i = 0; i < nw; ++i) s += red[e][i];
+    atomicAdd(out + j, s);
   }
 }
 
@@ -406,6 +461,7 @@ struct FirstArgs {
   T* db;          // [N]
   long long Np;
   int pts_per_block;
+  double* omega_grad;  // dW with trainable frequencies: fp64 accumulators of dLoss/d omega (see omega_flush)
 };
 
 // Z_1[c][p][n] = sum_f seed_c[p][f] W[f][n] (+ b[n] on the value channel)
@@ -426,16 +482,24 @@ __global__ void __launch_bounds__(256) k_first_fwd(FirstArgs<T> g) {
 }
 
 // dW_1[f][n] += sum_{c,p} seed_c[p][f] Zbar_1[c][p][n] ;  db_1[n] += sum_p Zbar_1[0][p][n]
-template <typename T, int KMAX>
+// OMEGA (trainable frequencies): also dLoss/d omega of feature f = sum_{c,p,n} dseed_c[p][f]/d omega Zbar_1[c][p][n] W[f][n],
+// each thread's share (its column n) reduced by omega_flush
+template <typename T, int KMAX, bool OMEGA = false>
 __global__ void __launch_bounds__(256) k_first_dw(FirstArgs<T> g) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
-  if (n >= g.N) return;
+  const bool n_ok = n < g.N;
+  if (!OMEGA && !n_ok) return;
   const long long p_begin = (long long)blockIdx.y * g.pts_per_block;
   long long p_end = p_begin + g.pts_per_block;
   if (p_end > g.Np) p_end = g.Np;
-  T acc[THIN_MAXF];
+  if (!n_ok) p_end = p_begin;
+  T acc[THIN_MAXF], oacc[THIN_MAXF], w[THIN_MAXF];
 #pragma unroll
-  for (int f = 0; f < THIN_MAXF; ++f) acc[f] = T(0);
+  for (int f = 0; f < THIN_MAXF; ++f) {
+    acc[f] = T(0);
+    oacc[f] = T(0);
+    w[f] = (OMEGA && n_ok && f < g.nf) ? g.W[(long long)f * g.N + n] : T(0);
+  }
   T dbacc = T(0);
   for (long long p = p_begin; p < p_end; ++p) {
     const T* zb = g.Zbar + p * g.ldzb + n;
@@ -446,13 +510,72 @@ __global__ void __launch_bounds__(256) k_first_dw(FirstArgs<T> g) {
         T a = T(0);
         produce_a<T, KMAX>(g.A, g.J, p, f, true, [&](int c, T v) { a += v * zb[(long long)c * g.zbplane]; });
         acc[f] += a;
+        if (OMEGA && g.A.seed.omega_idx[f] >= 0) {
+          T d = T(0);
+          produce_dseed<T, KMAX>(g.A, g.J, p, f, [&](int c, T v) { d += v * zb[(long long)c * g.zbplane]; });
+          oacc[f] += d * w[f];
+        }
       }
     }
   }
+  if (n_ok) {
 #pragma unroll
-  for (int f = 0; f < THIN_MAXF; ++f)
-    if (f < g.nf) atomicAdd(g.dW + (long long)f * g.N + n, acc[f]);
-  atomicAdd(g.db + n, dbacc);
+    for (int f = 0; f < THIN_MAXF; ++f)
+      if (f < g.nf) atomicAdd(g.dW + (long long)f * g.N + n, acc[f]);
+    atomicAdd(g.db + n, dbacc);
+  }
+  if constexpr (OMEGA) omega_flush<T, THIN_MAXF>(oacc, g.nf, g.A.seed.omega_idx, g.omega_grad);
+}
+
+// dLoss/d omega where the seeds' weight gradients come from the generic dW GEMM (more than THIN_MAXF features, gated
+// networks): every GEMM q that reads the seeds (Zbar_q = adjoint of its output, W_q = its [nf][N_q] weights) adds
+//   sum_{c,p,f} dseed_c[p][f]/d omega_f  sum_n Zbar_q[c][p][n] W_q[f][n].
+// One warp per point (grid-stride), lanes along n; shares reduced by omega_flush.
+template <typename T>
+struct OmegaArgs {
+  AOperand<T> A;  // A_SEED
+  JetLayout J;
+  int nf;
+  int n_cons;  // GEMMs reading the seeds: layer 1, + embed_u / embed_v of a ModifiedMLP without an embedding layer
+  const T* Zbar[3];
+  int ldzb[3];
+  long long zbplane[3];
+  const T* W[3];
+  int N[3];
+  long long Np;
+  double* omega_grad;
+};
+
+template <typename T, int KMAX>
+__global__ void __launch_bounds__(256) k_omega_grad(OmegaArgs<T> g) {
+  T part[PPSCI_MAX_FEAT];
+  for (int f = 0; f < PPSCI_MAX_FEAT; ++f) part[f] = T(0);
+  const int lane = threadIdx.x & 31;
+  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+  for (long long p = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); p < g.Np; p += warps) {
+    for (int f = 0; f < g.nf; ++f) {
+      if (g.A.seed.omega_idx[f] < 0) continue;
+      T acc = T(0);
+      produce_dseed<T, KMAX>(g.A, g.J, p, f, [&](int c, T d) {
+        T a = T(0);
+        for (int q = 0; q < g.n_cons; ++q) {
+          const T* zb = g.Zbar[q] + (long long)c * g.zbplane[q] + p * g.ldzb[q];
+          const T* w = g.W[q] + (long long)f * g.N[q];
+          for (int n = lane; n < g.N[q]; n += 32) a += zb[n] * w[n];
+        }
+        acc += d * a;
+      });
+      part[f] += acc;
+    }
+  }
+  omega_flush<T, PPSCI_MAX_FEAT>(part, g.nf, g.A.seed.omega_idx, g.omega_grad);
+}
+
+// grads[j] += acc[j]: the fp64 dLoss/d omega accumulators of a call into the caller's gradient buffer
+template <typename T>
+__global__ void k_omega_finish(const double* acc, T* grads, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) grads[i] += T(acc[i]);
 }
 
 template <typename T>

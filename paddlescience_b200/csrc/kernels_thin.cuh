@@ -30,6 +30,23 @@ __device__ __forceinline__ void stage_seeds(const FirstArgs<float>& g, long long
   }
 }
 
+// d seed / d omega of PB points -> shared memory  sD[pt][f][c]  (zero for the features with a fixed frequency)
+template <class L>
+__device__ __forceinline__ void stage_dseeds(const FirstArgs<float>& g, long long p0, float (*sD)[THIN_MAXF][L::CS]) {
+  for (int idx = threadIdx.x; idx < PB * g.nf; idx += blockDim.x) {
+    const int pt = idx / g.nf, f = idx - pt * g.nf;
+    const long long p = p0 + pt;
+    if (p < g.Np && g.A.seed.omega_idx[f] >= 0) {
+      produce_dseed<float, L::KM>(g.A, g.J, p, f, [&](int c, float v) {
+        if (c < L::CS) sD[pt][f][c] = v;
+      });
+    } else {
+#pragma unroll
+      for (int c = 0; c < L::CS; ++c) sD[pt][f][c] = 0.f;
+    }
+  }
+}
+
 // Z_1[c][p][n] = sum_f seed_c[p][f] W[f][n] (+ b[n] on the value channel).  Block = PB points x all columns.
 template <class L>
 __global__ void __launch_bounds__(256) k_first_fwd_v(FirstArgs<float> g) {
@@ -72,10 +89,14 @@ __global__ void __launch_bounds__(256) k_first_fwd_v(FirstArgs<float> g) {
 
 // dW_1[f][n] += sum_{c,p} seed_c[p][f] Zbar_1[c][p][n] ;  db_1[n] += sum_p Zbar_1[0][p][n]
 // grid (ceil(N / 256), ceil(Np / pts_per_block)), pts_per_block a multiple of PB.
-template <class L>
+// OMEGA (trainable frequencies): in the same pass over Zbar_1, dLoss/d omega of feature f
+//   = sum_{c,p} dseed_c[p][f]/d omega  sum_n Zbar_1[c][p][n] W[f][n]
+// (d seed / d omega staged beside the seeds, each thread's 4 columns accumulated in fp32, reduced by omega_flush)
+template <class L, bool OMEGA = false>
 __global__ void __launch_bounds__(256) k_first_dw_v(FirstArgs<float> g) {
   constexpr int CS = L::CS;
   __shared__ float sS[PB][THIN_MAXF][CS];
+  __shared__ float sD[OMEGA ? PB : 1][THIN_MAXF][CS];
   __shared__ float red[3][64][4];
   const int tid = threadIdx.x;
   const int nq = blockIdx.x * 64 + (tid & 63), lane4 = tid >> 6;
@@ -88,9 +109,19 @@ __global__ void __launch_bounds__(256) k_first_dw_v(FirstArgs<float> g) {
   for (int f = 0; f <= THIN_MAXF; ++f)
 #pragma unroll
     for (int t = 0; t < 4; ++t) acc[f][t] = 0.f;
+  float w[OMEGA ? THIN_MAXF : 1][4], oacc[THIN_MAXF];
+  if constexpr (OMEGA) {
+#pragma unroll
+    for (int f = 0; f < THIN_MAXF; ++f) {
+      oacc[f] = 0.f;
+#pragma unroll
+      for (int t = 0; t < 4; ++t) w[f][t] = (n_ok && f < g.nf) ? __ldg(g.W + (long long)f * g.N + 4 * nq + t) : 0.f;
+    }
+  }
   for (long long p0 = p_begin; p0 < p_end; p0 += PB) {
     __syncthreads();
     stage_seeds<L>(g, p0, sS);
+    if constexpr (OMEGA) stage_dseeds<L>(g, p0, sD);
     __syncthreads();
     if (!n_ok) continue;
     for (int pt = lane4; pt < PB; pt += 4) {
@@ -112,6 +143,21 @@ __global__ void __launch_bounds__(256) k_first_dw_v(FirstArgs<float> g) {
             for (int t = 0; t < 4; ++t) acc[f][t] += sv * f4c(z[c], t);
           }
         }
+      if constexpr (OMEGA) {
+#pragma unroll
+        for (int f = 0; f < THIN_MAXF; ++f)
+          if (f < g.nf && g.A.seed.omega_idx[f] >= 0) {
+            float d = 0.f;
+#pragma unroll
+            for (int c = 0; c < CS; ++c) {
+              float zw = 0.f;
+#pragma unroll
+              for (int t = 0; t < 4; ++t) zw += f4c(z[c], t) * w[f][t];
+              d += sD[pt][f][c] * zw;
+            }
+            oacc[f] += d;
+          }
+      }
     }
   }
   // reduce the four point lanes, then one atomic per (f, n)
@@ -131,6 +177,7 @@ __global__ void __launch_bounds__(256) k_first_dw_v(FirstArgs<float> g) {
       }
     }
   }
+  if constexpr (OMEGA) omega_flush<float, THIN_MAXF>(oacc, g.nf, g.A.seed.omega_idx, g.omega_grad);
 }
 
 // Y[c][p][j] = sum_k act_jets(Z_{L-1})[c][p][k] W[k][j] (+ b[j] on the value channel); one warp per point,

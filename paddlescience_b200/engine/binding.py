@@ -90,6 +90,8 @@ class PlanSpec(C.Structure):
         ("pgrad_aux", C.c_int32 * MAX_PGRAD),
         ("pgrad_reg", C.c_int32 * MAX_PGRAD),
         ("gated", C.c_int32),
+        ("n_omega", C.c_int32),
+        ("feat_omega_param", C.c_int32 * MAX_FEAT),
     ]
 
 

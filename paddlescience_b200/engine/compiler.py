@@ -60,6 +60,10 @@ class NetSpec:
     # 2: PirateNet (mlp.py:617-624, 800-809): layer 1 is the Fourier embedding, U / V read its output, then blocks of three
     #    layers (gate, gate, x <- alpha h + (1 - alpha) x)
     gated: int = 0
+    # trainable PeriodEmbedding frequencies (ppsci_plan_spec.feat_omega_param): feature f reads omega_j, j =
+    # feat_omega_param[f] >= 0, from the LAST n_omega entries of the parameter buffer (-1 / None: feat_omega[f])
+    feat_omega_param: Optional[List[int]] = None
+    n_omega: int = 0
 
     @property
     def n_params(self) -> int:
@@ -74,7 +78,7 @@ class NetSpec:
             n += sum(hidden)
         elif self.act == "swish_b":  # one beta per layer
             n += len(hidden)
-        return n
+        return n + self.n_omega
 
 
 @dataclass

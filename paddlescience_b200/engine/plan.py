@@ -65,10 +65,13 @@ class ResidualPlan:
         self.dense_in = bool(getattr(net, "dense_in", False))
         s.dense_in = 1 if self.dense_in else 0
         if not self.dense_in:
+            omega_param = getattr(net, "feat_omega_param", None) or [-1] * s.n_feat
             for f in range(s.n_feat):
                 s.feat_src[f] = net.feat_src[f]
                 s.feat_kind[f] = net.feat_kind[f]
                 s.feat_omega[f] = net.feat_omega[f]
+                s.feat_omega_param[f] = omega_param[f]  # trainable frequency index (read from params), or -1
+            s.n_omega = int(getattr(net, "n_omega", 0) or 0)
         s.n_layers = len(net.widths) - 1
         for i, w in enumerate(net.widths):
             s.widths[i] = w
