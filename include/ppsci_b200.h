@@ -290,6 +290,80 @@ int ppsci_b200_deeponet_head(int32_t dtype, int32_t act, const void* b, const vo
                              const void* label, const void* weight, int64_t n, int32_t n_features, double coef,
                              void* g_out, double* loss_acc, void* bbar, void* tbar, void* dbias, void* stream);
 
+/* Two-phase calls for plans WITH input derivatives (any C), in place only: jets_fwd_keep runs the forward as a training
+ * call does and leaves the output jets in the workspace, [C][n][ld] planes at plan_stash_offset(plan, n_points, n_layers)
+ * (ld = n_out rounded up to a multiple of 4, plane stride n_points * ld); the caller writes the adjoints of ALL C channels
+ * into the planes of the same layout at plan_stash_offset(plan, n_points, 300), then jets_bwd_kept runs only the adjoint
+ * from the stash and accumulates into grads (no seeding of the value channel: Ybar is used as the caller left it).
+ * Same rules as values_fwd_keep / values_bwd_kept: at most plan_chunk_points points, the same inputs / params /
+ * workspace in both calls, nothing else using the workspace in between.  Not for gated networks. */
+int ppsci_b200_jets_fwd_keep(ppsci_plan* plan, const void* const* x_cols, const void* const* aux_cols, int64_t n_points,
+                             const void* params, void* workspace, size_t workspace_bytes, void* stream);
+int ppsci_b200_jets_bwd_kept(ppsci_plan* plan, const void* const* x_cols, const void* const* aux_cols, int64_t n_points,
+                             const void* params, void* grads, void* workspace, size_t workspace_bytes, void* stream);
+
+/* DeepONet residual head on Taylor jets — physics-informed DeepONet (Wang, Wang & Perdikaris 2021): residuals that
+ * differentiate G(u)(y) = sum_i branch_i(u) act(trunk_i(y)) + b with respect to the trunk coordinate y, as the reference
+ * trains through autograd (jacobian / hessian of G w.r.t. y).  The trunk net carries jets along y (one direction,
+ * K = dir_order <= 4, C = 1 + K channels; n_dir = 0: values only), the branch net values only.  The residual program
+ * is the one of ppsci_plan_spec for a network with n_out = 1 and n_in = 1: before it runs
+ *   r[c] = G_c (channel c of G's jets, c < C),  r[C] = y,  r[C + 1 + a] = auxiliary column a.
+ * Per pair the head forms G_c, runs the program, accumulates the per-slot MSE and writes the adjoints of both
+ * sub-networks' outputs:  bbar_i = sum_c Gbar_c A_c[i],  tbar = adjoint of A = act(t) for the output-jet adjoints
+ * b_i Gbar_c (all C channels),  dbias += Gbar_0. */
+typedef struct ppsci_deeponet_head_spec {
+  int32_t dtype;
+  int32_t act; /* trunk activation (PPSCI_ACT_*, none with a trainable parameter) */
+  int32_t n_dir; /* 0 or 1 */
+  int32_t dir_order; /* 1 .. PPSCI_MAX_ORDER when n_dir == 1 */
+  int32_t n_aux;
+  int32_t n_reg;
+  int32_t n_ops;
+  const int32_t* prog; /* copied at create */
+  int32_t n_consts;
+  const double* consts; /* copied at create */
+  int32_t n_res;
+  int32_t res_reg[PPSCI_MAX_RES];
+  int32_t n_grad;
+  const int32_t* grad_res; /* copied at create */
+  const int32_t* grad_in;  /* register index < C, sorted */
+  const int32_t* grad_reg;
+} ppsci_deeponet_head_spec;
+
+/* One call of the head over n pairs.  b: branch outputs [n][ldb]; t: trunk output jets [C][n][ldt], plane stride
+ * tplane (both as jets_fwd_keep leaves them: they are read in place).  The columns y_col, aux_cols, label_cols,
+ * weight_cols and residual_out are indexed from x_off.  coef[k] = loss weight of slot k (/ n_norm for "mean").
+ * loss_acc: n_res device doubles, ACCUMULATED, or NULL.  bbar / tbar: the adjoints, same layouts as b / t (may be the
+ * stash_offset 300 planes of the two plans), both or neither; NULL = forward only (residual_out / loss_acc).  dbias:
+ * device scalar, accumulated, or NULL. */
+typedef struct ppsci_deeponet_jet_args {
+  const void* b;
+  int32_t ldb;
+  const void* t;
+  int32_t ldt;
+  int64_t tplane;
+  int64_t n;
+  int32_t n_features;
+  const void* bias;
+  const void* y_col;
+  const void* aux_cols[PPSCI_MAX_IN];
+  int64_t x_off;
+  const void* label_cols[PPSCI_MAX_RES];
+  double label_const[PPSCI_MAX_RES];
+  const void* weight_cols[PPSCI_MAX_RES];
+  double coef[PPSCI_MAX_RES];
+  void* residual_out[PPSCI_MAX_RES];
+  double* loss_acc;
+  void* bbar;
+  void* tbar;
+  void* dbias;
+} ppsci_deeponet_jet_args;
+
+typedef struct ppsci_deeponet_head ppsci_deeponet_head;
+int ppsci_b200_deeponet_jet_head_create(const ppsci_deeponet_head_spec* spec, ppsci_deeponet_head** out);
+int ppsci_b200_deeponet_jet_head_run(const ppsci_deeponet_head* head, const ppsci_deeponet_jet_args* args, void* stream);
+void ppsci_b200_deeponet_jet_head_destroy(ppsci_deeponet_head* head);
+
 /* Device-side collocation sampling — replaces, for axis-aligned boxes, the per-step numpy RNG + host-to-device copy of
  * ContinuousNamedArrayDataset.__iter__ (ppsci/data/dataset/array_dataset.py:208-228).  out_cols[d][i] = lo[d] +
  * (hi[d] - lo[d]) * U(seed; offset + i, d), U in [0, 1) from Philox4x32-10 (counter-based: the same (seed, offset)

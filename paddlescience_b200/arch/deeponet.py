@@ -4,17 +4,24 @@ Both sub-networks run in the native kernels (values only, C = 1): the branch net
 matrix as a dense first-layer operand (``dense_in``), the trunk net its coordinate column as an input seed.  The
 combination, the loss and their derivatives are elementwise work on ``[N, num_features]`` done with torch on the
 device; the weight gradients of the two MLPs come from ``ppsci_b200_values_fwd_bwd`` fed with dL/d(branch),
-dL/d(trunk).  One flat parameter buffer  [branch | trunk | b]  so the flat optimizers apply unchanged."""
+dL/d(trunk).  One flat parameter buffer  [branch | trunk | b]  so the flat optimizers apply unchanged.
+
+Physics-informed constraints (expressions that differentiate G with respect to the trunk coordinate) take the jet path:
+the trunk net carries Taylor jets along y, the residual program runs in ``k_deeponet_jet_head`` between the two
+sub-networks' forward and adjoint passes (``jets_fwd_keep`` / ``jets_bwd_kept``)."""
 from __future__ import annotations
 
+import ctypes as C
 import math
 from collections import OrderedDict
 from typing import Dict, Tuple, Union
 
+import sympy as sp
 import torch
+from sympy.core.function import AppliedUndef
 from torch import nn
 
-from ..engine.compiler import NetSpec, compile_residuals
+from ..engine.compiler import CompiledResidual, NetSpec, compile_residuals
 from . import activation as act_mod
 from . import base
 from .mlp import Reparam, hidden_sizes, stack_offsets
@@ -93,6 +100,8 @@ class DeepONet(base.Arch):
         self.flat = nn.Parameter(torch.zeros(off, dtype=dtype))
         self.reset_parameters()
         self._plans = None
+        self._jet_heads = {}  # residual sets of physics-informed constraints -> _JetHead
+        self._g_of_uy = sp.Function(G_key)(sp.Symbol(u_key), sp.Symbol(y_key))  # a label on G with no expression
 
     # ---- parameters ------------------------------------------------------------------------------
     def _layers(self):
@@ -215,20 +224,27 @@ class DeepONet(base.Arch):
             out = self._output_transform(x, out)
         return out
 
-    def fused_train_forward(self, loss_fn, input_dict, label_dict, weight_dict) -> Dict[str, torch.Tensor]:
+    def fused_train_forward(self, loss_fn, input_dict, label_dict, weight_dict, output_expr=None,
+                            extra_keys=()) -> Dict[str, torch.Tensor]:
         """Loss of one constraint + accumulation of its gradient into ``self.flat.grad``.
 
         Replaces expression.py:96-129 + train.py:158 for this model without any framework autograd graph: native forward
         of both sub-nets with the adjoint's stash kept (``values_fwd_keep``), ONE head kernel for the product, the MSE and
         the two adjoint seeds dL/d(branch), dL/d(trunk) (``ppsci_b200_deeponet_head``), native adjoints of both sub-nets
         from the kept stash (``values_bwd_kept`` — the forward is not recomputed).  Batches larger than the plans'
-        workspace chunk are processed slice by slice."""
+        workspace chunk are processed slice by slice.
+
+        ``output_expr`` (the constraint's expressions) with a key that is not a model output selects the residual path
+        of physics-informed DeepONet: the expressions may differentiate G with respect to the trunk coordinate and use
+        extra input columns (``extra_keys``); see ``_jet_train_forward``."""
         from ..engine import binding as B
 
         if self._input_transform is not None or self._output_transform is not None:
             raise NotImplementedError("input / output transforms are not supported on the fused DeepONet training path")
         if type(loss_fn).__name__ != "MSELoss":
             raise NotImplementedError(f"{type(loss_fn).__name__} has no fused head kernel; only MSELoss is on the hot path")
+        if output_expr is not None and any(k not in self.output_keys for k in output_expr):
+            return self._jet_train_forward(loss_fn, input_dict, label_dict, weight_dict, output_expr, extra_keys)
         flat = self.flat
         if flat.grad is None:
             flat.grad = torch.zeros_like(flat.data)
@@ -281,3 +297,207 @@ class DeepONet(base.Arch):
             pt.values_bwd_kept(ptr_, gtr, tbar)
         self._finish_sub_grads()
         return {key: loss_acc[0].to(dt)}
+
+    # ---- physics-informed DeepONet: residuals on the trunk coordinate's Taylor jets -----------------
+    def _jet_residuals(self, exprs: Dict[str, object], extra_keys) -> Dict[str, sp.Basic]:
+        """sympy residuals of ``exprs`` over G(y): traced with G = G(u, y), then checked to use neither a derivative with
+        respect to u nor u itself (after G(u, y) -> G(y) either would silently read as 0)."""
+        from ..equation.pde.base import lookup_parameter
+        from ..utils import symbolic
+
+        u, y, g = self.u_key, self.y_key, self.output_keys[0]
+        usym, ysym = sp.Symbol(u), sp.Symbol(y)
+        out = {}
+        for name, e in exprs.items():
+            if isinstance(e, symbolic.CompiledExpr):
+                e = e.expr
+            elif not isinstance(e, sp.Basic):
+                if not callable(e):
+                    raise TypeError(f"output_expr['{name}'] must be a sympy expression or a callable, got {type(e)}")
+                e = symbolic.trace_to_sympy(e, (u, y), (g,), list(extra_keys))
+            e = sp.sympify(e)
+            for d in e.atoms(sp.Derivative):
+                if any(str(v) == u for v, _ in d.variable_count):
+                    raise NotImplementedError(f"DeepONet expression '{name}': derivatives with respect to the branch input "
+                                              f"'{u}' are not supported (only the trunk coordinate '{y}')")
+            e = e.replace(lambda a: isinstance(a, AppliedUndef) and a.func.__name__ == g, lambda a: sp.Function(g)(ysym))
+            if usym in e.free_symbols:
+                raise NotImplementedError(f"DeepONet expression '{name}' uses the branch input '{u}' itself; only G, its "
+                                          f"derivatives with respect to '{y}', '{y}' and extra input columns are supported")
+            learnable = sorted(str(s_) for s_ in e.free_symbols if lookup_parameter(str(s_)) is not None)
+            if learnable:
+                raise NotImplementedError(f"DeepONet expression '{name}': learnable equation parameters {learnable} are "
+                                          "not supported")
+            out[name] = e
+        return out
+
+    def _jet_head(self, exprs: Dict[str, object], extra_keys) -> "_JetHead":
+        """The compiled residual set of ``exprs`` with its trunk plan and native head for the current dtype (cached)."""
+        key = (tuple((name, id(e)) for name, e in exprs.items()), tuple(extra_keys), self.flat.dtype)
+        hit = self._jet_heads.get(key)
+        if hit is None or any(a is not b for a, b in zip(hit.sources, exprs.values())):
+            hit = _JetHead(self, self._jet_residuals(exprs, extra_keys), list(exprs.values()))
+            self._jet_heads[key] = hit
+        return hit
+
+    def _jet_run(self, head: "_JetHead", input_dict, labels, weights, coefs, loss_acc, residual_out, train: bool):
+        """Chunked forward of both sub-networks with the adjoint's stash kept (``jets_fwd_keep``), the jet head
+        (``deeponet_jet_head_run``) and, when ``train``, both adjoints from the stash (``jets_bwd_kept``)."""
+        from ..engine import binding as B
+
+        flat = self.flat
+        dt, dev = flat.dtype, flat.device
+        u = input_dict[self.u_key].to(dt)
+        y = input_dict[self.y_key].to(dt).reshape(-1).contiguous()
+        if dev != u.device:
+            raise ValueError(f"inputs are on {u.device}, parameters are on {dev}")
+        n = u.shape[0]
+        cr = head.compiled
+        aux = [input_dict[k].to(dt).reshape(-1).contiguous() for k in cr.aux_keys]
+        pb = self._get_plans()[0]
+        pt = head.trunk_plan
+        lib = pb.lib
+        pbr, ptr_ = self._sub_params()
+        gbr, gtr = self._sub_grads() if train else (None, None)
+        bias = flat.data[self._bias_off: self._bias_off + 1] if self.use_bias else None
+        dbias = flat.grad[self._bias_off: self._bias_off + 1] if (train and self.use_bias) else None
+        a = B.DeepONetJetArgs()
+        a.n_features = self.num_features
+        a.bias = bias.data_ptr() if bias is not None else None
+        a.y_col = y.data_ptr()
+        for i, t in enumerate(aux):
+            a.aux_cols[i] = t.data_ptr()
+        for k in range(len(cr.names)):
+            lab = labels[k]
+            if torch.is_tensor(lab):
+                a.label_cols[k] = lab.data_ptr()
+            else:
+                a.label_const[k] = float(lab)
+            a.weight_cols[k] = weights[k].data_ptr() if weights[k] is not None else None
+            a.coef[k] = coefs[k]
+            a.residual_out[k] = residual_out[k].data_ptr() if residual_out is not None else None
+        a.loss_acc = loss_acc.data_ptr() if loss_acc is not None else None
+        a.dbias = dbias.data_ptr() if dbias is not None else None
+        chunk = min(pb.chunk_points, pt.chunk_points)
+        stream = torch.cuda.current_stream(dev).cuda_stream if dev.type == "cuda" else 0
+        for s0 in range(0, n, chunk):
+            sl = slice(s0, min(n, s0 + chunk))
+            a.b, bbar, a.ldb, _ = pb.jets_fwd_keep({self.u_key: u[sl]}, pbr)
+            a.t, tbar, a.ldt, a.tplane = pt.jets_fwd_keep({self.y_key: y[sl]}, ptr_)
+            a.n = sl.stop - s0
+            a.x_off = s0
+            a.bbar, a.tbar = (bbar, tbar) if train else (None, None)
+            lib.check(lib.lib.ppsci_b200_deeponet_jet_head_run(head.handle, C.byref(a), stream), "deeponet_jet_head_run")
+            if train:
+                pb.jets_bwd_kept(pbr, gbr)
+                pt.jets_bwd_kept(ptr_, gtr)
+        if train:
+            self._finish_sub_grads()
+
+    def _jet_train_forward(self, loss_fn, input_dict, label_dict, weight_dict, output_expr, extra_keys):
+        """Physics-informed DeepONet: the losses of ``output_expr``'s slots (in the order of ``label_dict``; a label key
+        without an expression is G itself), whose residuals may differentiate G with respect to the trunk coordinate,
+        and their gradient accumulated into ``self.flat.grad``.  Per slot: label column or constant, weight column (times
+        ``area``), reduction and MSELoss weight, as mse.py:82-106."""
+        flat = self.flat
+        if flat.grad is None:
+            flat.grad = torch.zeros_like(flat.data)
+        dt, dev = flat.dtype, flat.device
+        g_key = self.output_keys[0]
+        names = list(label_dict)
+        for k in names:
+            if k not in output_expr and k != g_key:
+                raise KeyError(f"label '{k}' has neither an output expression nor a model output")
+        exprs = {k: output_expr[k] if k in output_expr else self._g_of_uy for k in names}
+        head = self._jet_head(exprs, extra_keys)
+        n = input_dict[self.u_key].shape[0]
+        red = getattr(loss_fn, "reduction", "mean")
+        area = input_dict["area"].to(dt).reshape(-1) if "area" in input_dict else None
+        labels, weights, coefs = [], [], []
+        for k in names:
+            lab = label_dict[k]
+            if torch.is_tensor(lab) and lab.numel() == n:
+                labels.append(lab.to(dev, dt).reshape(-1).contiguous())
+            else:
+                labels.append(float(lab.reshape(-1)[0]) if torch.is_tensor(lab) else float(lab))
+            w = weight_dict.get(k) if weight_dict else None
+            if w is not None:
+                w = (w.to(dev, dt).reshape(-1) if torch.is_tensor(w) else torch.full((1,), float(w), dtype=dt, device=dev))
+            if area is not None:  # mse.py:92-93
+                w = area if w is None else w * area
+            weights.append(w.expand(n).contiguous() if w is not None else None)
+            coefs.append(float(loss_fn.weight_of(k) if hasattr(loss_fn, "weight_of") else 1.0) * (1.0 / n if red == "mean" else 1.0))
+        loss_acc = torch.zeros(len(names), dtype=torch.float64, device=dev)
+        self._jet_run(head, input_dict, labels, weights, coefs, loss_acc, None, train=True)
+        return {k: loss_acc[i].to(dt) for i, k in enumerate(names)}
+
+    def evaluate_expressions(self, exprs: Dict[str, object], input_dict, extra_keys=()) -> Dict[str, torch.Tensor]:
+        """Values [N, 1] of expressions over G, its derivatives with respect to the trunk coordinate, the inputs and
+        extra columns (eval / visualisation), from one forward-only run of the jet head."""
+        first = input_dict[self.u_key]
+        if self._input_transform is not None or self._output_transform is not None:
+            raise NotImplementedError("input / output transforms are not supported on DeepONet expressions")
+        head = self._jet_head(exprs, extra_keys)
+        n = first.shape[0]
+        out = [torch.empty((n, 1), dtype=self.flat.dtype, device=first.device) for _ in exprs]
+        k = len(out)
+        self._jet_run(head, input_dict, [0.0] * k, [None] * k, [0.0] * k, None, out, train=False)
+        return dict(zip(exprs, out))
+
+
+class _JetHead:
+    """One compiled DeepONet residual set for one dtype: the register program over G's jets along the trunk coordinate
+    (compiled on a one-input, one-output network), the trunk plan built with that program's jet layout, and the native
+    head (``ppsci_b200_deeponet_jet_head_create``) holding the program on the device."""
+
+    def __init__(self, model: DeepONet, exprs: Dict[str, sp.Basic], sources):
+        from ..engine import binding as B
+        from ..engine.plan import ResidualPlan, _dtype_id
+
+        self.sources = sources  # keeps the cache key's ids alive
+        g_key, y_key = model.output_keys[0], model.y_key
+        net = NetSpec((y_key,), (g_key,), [0], [0], [0.0], [1, 1], model.trunk_activation)
+        cr = compile_residuals(net, exprs)
+        if len(cr.names) > B.MAX_RES:
+            raise NotImplementedError(f"more than {B.MAX_RES} residuals per constraint")
+        if len(cr.aux_keys) > B.MAX_IN:
+            raise NotImplementedError(f"more than {B.MAX_IN} auxiliary columns")
+        self.compiled = cr
+        trunk = CompiledResidual(net=model._trunk, names=[], dirs=cr.dirs, aux_keys=[], n_reg=0, prog=[], consts=[],
+                                 res_reg=[], grad_res=[], grad_in=[], grad_reg=[])
+        self.trunk_plan = ResidualPlan(trunk, model.flat.dtype, [], [])
+        self.lib = self.trunk_plan.lib
+        s = B.DeepONetHeadSpec()
+        s.dtype = _dtype_id(model.flat.dtype)
+        s.act = B.ACT_IDS[model.trunk_activation]
+        s.n_dir = len(cr.dirs)
+        s.dir_order = cr.dirs[0].order if cr.dirs else 0
+        s.n_aux = len(cr.aux_keys)
+        s.n_reg = cr.n_reg
+        s.n_ops = len(cr.prog)
+        self._prog = (C.c_int32 * max(1, 4 * len(cr.prog)))(*[x for op in cr.prog for x in op])
+        self._consts = (C.c_double * max(1, len(cr.consts)))(*cr.consts)
+        self._gres = (C.c_int32 * max(1, len(cr.grad_res)))(*cr.grad_res)
+        self._gin = (C.c_int32 * max(1, len(cr.grad_in)))(*cr.grad_in)
+        self._greg = (C.c_int32 * max(1, len(cr.grad_reg)))(*cr.grad_reg)
+        s.prog = C.cast(self._prog, C.POINTER(C.c_int32))
+        s.n_consts = len(cr.consts)
+        s.consts = C.cast(self._consts, C.POINTER(C.c_double))
+        s.n_res = len(cr.names)
+        for k, r in enumerate(cr.res_reg):
+            s.res_reg[k] = r
+        s.n_grad = len(cr.grad_res)
+        s.grad_res = C.cast(self._gres, C.POINTER(C.c_int32))
+        s.grad_in = C.cast(self._gin, C.POINTER(C.c_int32))
+        s.grad_reg = C.cast(self._greg, C.POINTER(C.c_int32))
+        handle = C.c_void_p()
+        self.lib.check(self.lib.lib.ppsci_b200_deeponet_jet_head_create(C.byref(s), C.byref(handle)), "deeponet_jet_head_create")
+        self.handle = handle
+
+    def __del__(self):
+        try:
+            if getattr(self, "handle", None):
+                self.lib.lib.ppsci_b200_deeponet_jet_head_destroy(self.handle)
+                self.handle = None
+        except Exception:
+            pass

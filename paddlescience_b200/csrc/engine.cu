@@ -201,6 +201,38 @@ static int op_arity(int op) {
   }
 }
 
+// registers, instructions, residual registers and the partials list of a residual program whose first n_inreg
+// registers are loaded before it runs, n_grad_in of them output-jet registers (plan_create, deeponet_jet_head_create)
+static int check_program(const std::string& what, int n_inreg, int n_grad_in, int n_reg, int n_ops, const int32_t* prog,
+                         int n_consts, int n_res, const int32_t* res_reg, int n_grad, const int32_t* grad_res,
+                         const int32_t* grad_in, const int32_t* grad_reg) {
+  if (n_reg < n_inreg || n_reg > PPSCI_MAX_REG) return fail(what + ": n_reg out of range (max 256)");
+  if (n_ops < 0 || (n_ops > 0 && !prog)) return fail(what + ": bad program");
+  for (int i = 0; i < n_ops; ++i) {
+    const int op = prog[4 * i], dst = prog[4 * i + 1], a = prog[4 * i + 2], b = prog[4 * i + 3];
+    const int ar = op_arity(op);
+    if (ar < 0) return fail(what + ": unknown opcode at op " + std::to_string(i));
+    if (dst < 0 || dst >= n_reg) return fail(what + ": dst register out of range at op " + std::to_string(i));
+    if (op == PPSCI_OP_CONST) {
+      if (a < 0 || a >= n_consts) return fail(what + ": const index out of range at op " + std::to_string(i));
+    } else {
+      if (a < 0 || a >= n_reg) return fail(what + ": src register out of range at op " + std::to_string(i));
+      if (ar == 2 && (b < 0 || b >= n_reg)) return fail(what + ": src register out of range at op " + std::to_string(i));
+    }
+  }
+  for (int k = 0; k < n_res; ++k)
+    if (res_reg[k] < 0 || res_reg[k] >= n_reg) return fail(what + ": res_reg out of range");
+  if (n_grad < 0) return fail(what + ": n_grad < 0");
+  if (n_grad > 0 && (!grad_res || !grad_in || !grad_reg)) return fail(what + ": null grad list");
+  for (int g = 0; g < n_grad; ++g) {
+    if (grad_res[g] < 0 || grad_res[g] >= n_res) return fail(what + ": grad_res out of range");
+    if (grad_in[g] < 0 || grad_in[g] >= n_grad_in) return fail(what + ": grad_in out of range");
+    if (grad_reg[g] < 0 || grad_reg[g] >= n_reg) return fail(what + ": grad_reg out of range");
+    if (g > 0 && grad_in[g] < grad_in[g - 1]) return fail(what + ": grad list must be sorted by grad_in");
+  }
+  return 0;
+}
+
 extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out) {
   if (!s || !out) return fail("plan_create: null argument");
   *out = nullptr;
@@ -251,33 +283,15 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
   if (C > RC) return fail("plan_create: too many jet channels (max 32)");
   const int n_out = s->widths[s->n_layers];
   if (s->n_aux < 0 || s->n_aux > PPSCI_MAX_IN) return fail("plan_create: n_aux out of range");
+  // a plan without residual program (a sub-network whose outputs a caller's head reads) has no register file
   const int n_inreg = C * n_out + s->n_in + s->n_aux;
-  if (s->n_reg < n_inreg || s->n_reg > PPSCI_MAX_REG) return fail("plan_create: n_reg out of range (max 256)");
   if (s->n_res < 0 || s->n_res > PPSCI_MAX_RES) return fail("plan_create: n_res out of range");
-  if (s->n_ops < 0 || (s->n_ops > 0 && !s->prog)) return fail("plan_create: bad program");
-  for (int i = 0; i < s->n_ops; ++i) {
-    const int op = s->prog[4 * i], dst = s->prog[4 * i + 1], a = s->prog[4 * i + 2], b = s->prog[4 * i + 3];
-    const int ar = op_arity(op);
-    if (ar < 0) return fail("plan_create: unknown opcode at op " + std::to_string(i));
-    if (dst < 0 || dst >= s->n_reg) return fail("plan_create: dst register out of range at op " + std::to_string(i));
-    if (op == PPSCI_OP_CONST) {
-      if (a < 0 || a >= s->n_consts) return fail("plan_create: const index out of range at op " + std::to_string(i));
-    } else {
-      if (a < 0 || a >= s->n_reg) return fail("plan_create: src register out of range at op " + std::to_string(i));
-      if (ar == 2 && (b < 0 || b >= s->n_reg)) return fail("plan_create: src register out of range at op " + std::to_string(i));
-    }
-  }
-  for (int k = 0; k < s->n_res; ++k) {
-    if (s->res_reg[k] < 0 || s->res_reg[k] >= s->n_reg) return fail("plan_create: res_reg out of range");
+  if ((s->n_ops != 0 || s->n_res != 0 || s->n_grad != 0) &&
+      check_program("plan_create", n_inreg, C * n_out, s->n_reg, s->n_ops, s->prog, s->n_consts, s->n_res, s->res_reg,
+                    s->n_grad, s->grad_res, s->grad_in, s->grad_reg))
+    return 1;
+  for (int k = 0; k < s->n_res; ++k)
     if (s->reduction[k] != PPSCI_REDUCE_MEAN && s->reduction[k] != PPSCI_REDUCE_SUM) return fail("plan_create: bad reduction");
-  }
-  if (s->n_grad < 0) return fail("plan_create: n_grad < 0");
-  for (int g = 0; g < s->n_grad; ++g) {
-    if (s->grad_res[g] < 0 || s->grad_res[g] >= s->n_res) return fail("plan_create: grad_res out of range");
-    if (s->grad_in[g] < 0 || s->grad_in[g] >= C * n_out) return fail("plan_create: grad_in out of range");
-    if (s->grad_reg[g] < 0 || s->grad_reg[g] >= s->n_reg) return fail("plan_create: grad_reg out of range");
-    if (g > 0 && s->grad_in[g] < s->grad_in[g - 1]) return fail("plan_create: grad list must be sorted by grad_in");
-  }
   if (s->n_pgrad < 0 || s->n_pgrad > PPSCI_MAX_PGRAD) return fail("plan_create: n_pgrad out of range");
   for (int g = 0; g < s->n_pgrad; ++g) {
     if (s->pgrad_res[g] < 0 || s->pgrad_res[g] >= s->n_res) return fail("plan_create: pgrad_res out of range");
@@ -1280,6 +1294,169 @@ extern "C" int ppsci_b200_deeponet_head(int32_t dtype, int32_t act, const void* 
     PPSCI_LAUNCH(k_deeponet_head<T>, dim3(blocks), dim3(256), 0, stream, (const T*)b, (const T*)t, (const T*)bias, act,
                  (const T*)label, (const T*)weight, (long long)n, n_features, coef, (T*)g_out, loss_acc, (T*)bbar, (T*)tbar,
                  (T*)dbias);
+    CK(cudaGetLastError());
+    return 0;
+  });
+}
+
+extern "C" int ppsci_b200_jets_fwd_keep(ppsci_plan* plan, const void* const* x_cols, const void* const* aux_cols, int64_t n_points,
+                                        const void* params, void* workspace, size_t workspace_bytes, void* stream) {
+  if (plan && n_points > plan->chunk) return fail("jets_fwd_keep: at most plan_chunk_points points per call");
+  CallArgs a;
+  memset(&a, 0, sizeof(a));
+  a.x_cols = x_cols;
+  a.aux_cols = aux_cols;
+  a.n_points = n_points;
+  a.n_norm = n_points;
+  a.params = params;
+  a.workspace = workspace;
+  a.workspace_bytes = workspace_bytes;
+  a.stream = stream;
+  a.phase = 1;
+  return dispatch(plan, a);
+}
+
+extern "C" int ppsci_b200_jets_bwd_kept(ppsci_plan* plan, const void* const* x_cols, const void* const* aux_cols, int64_t n_points,
+                                        const void* params, void* grads, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!grads) return fail("jets_bwd_kept: null grads");
+  if (!plan || !workspace || n_points <= 0) return fail("jets_bwd_kept: bad arguments");
+  CallArgs a;
+  memset(&a, 0, sizeof(a));
+  a.x_cols = x_cols;
+  a.aux_cols = aux_cols;
+  a.n_points = n_points;
+  a.n_norm = n_points;
+  a.params = params;
+  a.grads = grads;
+  a.workspace = workspace;
+  a.workspace_bytes = workspace_bytes;
+  a.stream = stream;
+  a.ybar_in = static_cast<unsigned char*>(workspace) + ppsci_b200_plan_stash_offset(plan, n_points, 300);  // in place: no seeding
+  a.phase = 2;
+  return dispatch(plan, a);
+}
+
+struct ppsci_deeponet_head {
+  ppsci_deeponet_head_spec spec;
+  JetLayout J;
+  int kmax = 1;
+  int* d_prog = nullptr;
+  double* d_consts = nullptr;
+  int* d_grad_res = nullptr;
+  int* d_grad_in = nullptr;
+  int* d_grad_reg = nullptr;
+};
+
+extern "C" void ppsci_b200_deeponet_jet_head_destroy(ppsci_deeponet_head* H) {
+  if (!H) return;
+  cudaFree(H->d_prog);
+  cudaFree(H->d_consts);
+  cudaFree(H->d_grad_res);
+  cudaFree(H->d_grad_in);
+  cudaFree(H->d_grad_reg);
+  delete H;
+}
+
+extern "C" int ppsci_b200_deeponet_jet_head_create(const ppsci_deeponet_head_spec* s, ppsci_deeponet_head** out) {
+  if (!s || !out) return fail("deeponet_jet_head_create: null argument");
+  *out = nullptr;
+  if (s->dtype != PPSCI_F32 && s->dtype != PPSCI_F64) return fail("deeponet_jet_head_create: dtype must be f32 or f64");
+  if (s->act < 0 || s->act > PPSCI_ACT_LAST) return fail("deeponet_jet_head_create: unknown activation");
+  if (act_has_param(s->act)) return fail("deeponet_jet_head_create: activations with a trainable parameter are not offered here");
+  if (s->n_dir != 0 && s->n_dir != 1) return fail("deeponet_jet_head_create: n_dir must be 0 or 1 (the trunk coordinate)");
+  if (s->n_dir == 1 && (s->dir_order < 1 || s->dir_order > PPSCI_MAX_ORDER))
+    return fail("deeponet_jet_head_create: dir_order out of range");
+  if (s->n_aux < 0 || s->n_aux > PPSCI_MAX_IN) return fail("deeponet_jet_head_create: n_aux out of range");
+  if (s->n_res < 1 || s->n_res > PPSCI_MAX_RES) return fail("deeponet_jet_head_create: n_res out of range");
+  const int C = 1 + (s->n_dir ? s->dir_order : 0);
+  if (check_program("deeponet_jet_head_create", C + 1 + s->n_aux, C, s->n_reg, s->n_ops, s->prog, s->n_consts, s->n_res,
+                    s->res_reg, s->n_grad, s->grad_res, s->grad_in, s->grad_reg))
+    return 1;
+  ppsci_deeponet_head* H = new ppsci_deeponet_head();
+  H->spec = *s;
+  H->spec.prog = nullptr;
+  H->spec.consts = nullptr;
+  H->spec.grad_res = H->spec.grad_in = H->spec.grad_reg = nullptr;
+  memset(&H->J, 0, sizeof(H->J));
+  H->J.C = C;
+  H->J.n_dir = s->n_dir;
+  H->J.dir_order[0] = s->n_dir ? s->dir_order : 0;
+  H->J.dir_base[0] = 1;
+  H->kmax = C - 1 <= 1 ? 1 : (C - 1 == 2 ? 2 : 4);
+  auto up = [&](const void* src, size_t bytes, void** dst) -> cudaError_t {
+    cudaError_t e = cudaMalloc(dst, bytes ? bytes : 16);
+    if (e != cudaSuccess) return e;
+    if (bytes) return cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice);
+    return cudaSuccess;
+  };
+  cudaError_t e = cudaSuccess;
+  if (e == cudaSuccess) e = up(s->prog, (size_t)s->n_ops * 16, (void**)&H->d_prog);
+  if (e == cudaSuccess) e = up(s->consts, (size_t)s->n_consts * 8, (void**)&H->d_consts);
+  if (e == cudaSuccess) e = up(s->grad_res, (size_t)s->n_grad * 4, (void**)&H->d_grad_res);
+  if (e == cudaSuccess) e = up(s->grad_in, (size_t)s->n_grad * 4, (void**)&H->d_grad_in);
+  if (e == cudaSuccess) e = up(s->grad_reg, (size_t)s->n_grad * 4, (void**)&H->d_grad_reg);
+  if (e != cudaSuccess) {
+    ppsci_b200_deeponet_jet_head_destroy(H);
+    return fail(std::string("deeponet_jet_head_create: device upload of the residual program failed: ") + cudaGetErrorString(e));
+  }
+  *out = H;
+  return 0;
+}
+
+extern "C" int ppsci_b200_deeponet_jet_head_run(const ppsci_deeponet_head* H, const ppsci_deeponet_jet_args* a, void* stream) {
+  if (!H || !a) return fail("deeponet_jet_head_run: null argument");
+  const ppsci_deeponet_head_spec& s = H->spec;
+  if (!a->b || !a->t || !a->y_col || a->n <= 0 || a->n_features <= 0 || a->x_off < 0)
+    return fail("deeponet_jet_head_run: bad arguments");
+  if (a->ldb < a->n_features || a->ldt < a->n_features || a->tplane < a->n * a->ldt)
+    return fail("deeponet_jet_head_run: row pitch or plane stride smaller than the features");
+  if ((a->bbar == nullptr) != (a->tbar == nullptr)) return fail("deeponet_jet_head_run: bbar and tbar must both be given or both be null");
+  for (int i = 0; i < s.n_aux; ++i)
+    if (!a->aux_cols[i]) return fail("deeponet_jet_head_run: null aux column " + std::to_string(i));
+  return with_dtype(s.dtype, "deeponet_jet_head_run", [&](auto zero) {
+    using T = decltype(zero);
+    DeepONetJetArgs<T> h;
+    memset(&h, 0, sizeof(h));
+    h.P.prog = H->d_prog;
+    h.P.consts = H->d_consts;
+    h.P.n_ops = s.n_ops;
+    h.P.n_reg = s.n_reg;
+    h.P.n_res = s.n_res;
+    for (int k = 0; k < s.n_res; ++k) h.P.res_reg[k] = s.res_reg[k];
+    h.P.n_grad = s.n_grad;
+    h.P.grad_res = H->d_grad_res;
+    h.P.grad_in = H->d_grad_in;
+    h.P.grad_reg = H->d_grad_reg;
+    h.J = H->J;
+    h.act = s.act;
+    h.b = (const T*)a->b;
+    h.ldb = a->ldb;
+    h.t = (const T*)a->t;
+    h.ldt = a->ldt;
+    h.tplane = a->tplane;
+    h.n = a->n;
+    h.F = a->n_features;
+    h.bias = (const T*)a->bias;
+    h.y_col = (const T*)a->y_col;
+    for (int i = 0; i < s.n_aux; ++i) h.aux_cols[i] = a->aux_cols[i];
+    h.n_aux = s.n_aux;
+    h.x_off = a->x_off;
+    for (int k = 0; k < s.n_res; ++k) {
+      h.label_cols[k] = a->label_cols[k];
+      h.label_const[k] = a->label_const[k];
+      h.weight_cols[k] = a->weight_cols[k];
+      h.coef[k] = a->coef[k];
+      h.residual_out[k] = a->residual_out[k];
+    }
+    h.loss_acc = a->loss_acc;
+    h.bbar = (T*)a->bbar;
+    h.tbar = (T*)a->tbar;
+    h.dbias = (T*)a->dbias;
+    const long long warps = a->n < 132LL * 64 ? a->n : 132LL * 64;  // 8 warps per block
+    const unsigned blocks = (unsigned)((warps + 7) / 8);
+    void (*k)(DeepONetJetArgs<T>) = H->kmax == 1 ? k_deeponet_jet_head<T, 1>
+                                   : H->kmax == 2 ? k_deeponet_jet_head<T, 2> : k_deeponet_jet_head<T, 4>;
+    PPSCI_LAUNCH(k, dim3(blocks), dim3(256), 0, stream, h);
     CK(cudaGetLastError());
     return 0;
   });

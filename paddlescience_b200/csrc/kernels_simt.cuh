@@ -930,6 +930,135 @@ __global__ void __launch_bounds__(256) k_deeponet_head(const T* b, const T* t, c
   }
 }
 
+// DeepONet head on the trunk coordinate's Taylor jets (physics-informed DeepONet).  Per pair p, with A = act(t) the
+// activation jets of the trunk features along the one direction y (C = 1 + K channels):
+//   G_c = sum_i b_i A_c[i] (+ bias on c = 0);  residual program on r[c] = G_c, r[C] = y, r[C + 1 + a] = aux a (as k_head
+//   with n_out = 1);  per-slot MSE;  Gbar_c from the program's partials;
+//   bbar_i = sum_c Gbar_c A_c[i] (the branch does not depend on y),  tbar = jet_adj(act, t, ybar_c = b_i Gbar_c),
+//   dbias += Gbar_0.
+// One warp per pair: lanes stride the features, the C sums are butterfly-reduced so every lane holds them and runs the
+// (uniform) program itself.  b / bbar are [n][ldb], t / tbar [C][n][ldt] with plane stride tplane; the adjoint is written
+// only when bbar != NULL (then tbar too), padding columns F .. ld-1 of both get zeros.
+template <typename T>
+struct DeepONetJetArgs {
+  HeadProgram P;
+  JetLayout J;
+  int act;
+  const T* b;
+  int ldb;
+  const T* t;
+  int ldt;
+  long long tplane;
+  long long n;
+  int F;
+  const T* bias;
+  const T* y_col;
+  const void* aux_cols[PPSCI_MAX_IN];
+  int n_aux;
+  long long x_off;  // chunk offset into y_col / aux / label / weight / residual columns
+  const void* label_cols[PPSCI_MAX_RES];
+  double label_const[PPSCI_MAX_RES];
+  const void* weight_cols[PPSCI_MAX_RES];
+  double coef[PPSCI_MAX_RES];
+  void* residual_out[PPSCI_MAX_RES];
+  double* loss_acc;  // [n_res] fp64 accumulators or null
+  T* bbar;
+  T* tbar;
+  T* dbias;
+};
+
+template <typename T, int KMAX>
+__global__ void __launch_bounds__(256) k_deeponet_jet_head(DeepONetJetArgs<T> h) {
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, wpb = blockDim.x >> 5;
+  const int C = h.J.C;
+  const T bias_v = h.bias ? h.bias[0] : T(0);
+  double part[PPSCI_MAX_RES];
+  for (int k = 0; k < h.P.n_res; ++k) part[k] = 0.0;
+  T db_part = T(0);
+  T r[PPSCI_MAX_REG];
+  for (long long p = (long long)blockIdx.x * wpb + wib; p < h.n; p += (long long)gridDim.x * wpb) {
+    const T* bp = h.b + p * h.ldb;
+    const T* tp = h.t + p * h.ldt;
+    T G[KMAX + 1];
+#pragma unroll
+    for (int c = 0; c <= KMAX; ++c) G[c] = T(0);
+    for (int i = lane; i < h.F; i += 32) {
+      T y0, s[6];
+      act_coef<T, KMAX>(h.act, tp[i], y0, s);
+      const T bi = bp[i];
+      G[0] += bi * y0;
+      jet_fwd<T, DynLay<KMAX>>(h.J, s, [&](int c) { return tp[(long long)c * h.tplane + i]; }, [&](int c, T v) {
+#pragma unroll
+        for (int q = 1; q <= KMAX; ++q)
+          if (c == q) G[q] += bi * v;
+      });
+    }
+#pragma unroll
+    for (int c = 0; c <= KMAX; ++c)
+      for (int o = 16; o > 0; o >>= 1) G[c] += __shfl_xor_sync(0xffffffffu, G[c], o);
+    G[0] += bias_v;
+#pragma unroll
+    for (int c = 0; c <= KMAX; ++c)
+      if (c < C) r[c] = G[c];
+    r[C] = h.y_col[h.x_off + p];
+    for (int a = 0; a < h.n_aux; ++a) r[C + 1 + a] = reinterpret_cast<const T*>(h.aux_cols[a])[h.x_off + p];
+    vm_run<T>(h.P, r);
+    T rb[PPSCI_MAX_RES];
+    for (int k = 0; k < h.P.n_res; ++k) {
+      const T res = r[h.P.res_reg[k]];
+      if (lane == 0 && h.residual_out[k]) reinterpret_cast<T*>(h.residual_out[k])[h.x_off + p] = res;
+      const T label = h.label_cols[k] ? reinterpret_cast<const T*>(h.label_cols[k])[h.x_off + p] : T(h.label_const[k]);
+      const T w = h.weight_cols[k] ? reinterpret_cast<const T*>(h.weight_cols[k])[h.x_off + p] : T(1);
+      const T e = res - label;
+      rb[k] = T(2) * e * w * T(h.coef[k]);
+      if (lane == 0) part[k] += (double)(w * e * e) * h.coef[k];
+    }
+    if (!h.bbar) continue;
+    T Gb[KMAX + 1];  // dLoss/dG_c; the grad list is sorted by grad_in (= c)
+#pragma unroll
+    for (int c = 0; c <= KMAX; ++c) {
+      Gb[c] = T(0);
+      for (int g = 0; g < h.P.n_grad; ++g)
+        if (h.P.grad_in[g] == c) Gb[c] += rb[h.P.grad_res[g]] * r[h.P.grad_reg[g]];
+    }
+    if (lane == 0) db_part += Gb[0];
+    T* bbp = h.bbar + p * h.ldb;
+    T* tbp = h.tbar + p * h.ldt;
+    for (int i = lane; i < h.ldb || i < h.ldt; i += 32) {
+      if (i >= h.F) {  // padding of the row pitch: the sub-networks' adjoints read zeros there
+        if (i < h.ldb) bbp[i] = T(0);
+        if (i < h.ldt)
+          for (int c = 0; c < C; ++c) tbp[(long long)c * h.tplane + i] = T(0);
+        continue;
+      }
+      T y0, s[6];
+      act_coef<T, KMAX + 1>(h.act, tp[i], y0, s);
+      const T bi = bp[i];
+      T bacc = Gb[0] * y0;
+      auto z = [&](int c) { return tp[(long long)c * h.tplane + i]; };
+      jet_fwd<T, DynLay<KMAX>>(h.J, s, z, [&](int c, T v) {
+#pragma unroll
+        for (int q = 1; q <= KMAX; ++q)
+          if (c == q) bacc += Gb[q] * v;
+      });
+      auto ybar = [&](int c) {
+        T g = Gb[0];
+#pragma unroll
+        for (int q = 1; q <= KMAX; ++q)
+          if (c == q) g = Gb[q];
+        return bi * g;
+      };
+      tbp[i] = jet_adj<T, DynLay<KMAX>>(h.J, s, z, ybar, [&](int c, T v) { tbp[(long long)c * h.tplane + i] = v; });
+      bbp[i] = bacc;
+    }
+  }
+  if (lane == 0) {
+    if (h.loss_acc)
+      for (int k = 0; k < h.P.n_res; ++k) atomicAdd(h.loss_acc + k, part[k]);
+    if (h.bbar && h.dbias) atomicAdd(h.dbias, db_part);
+  }
+}
+
 // Device-side collocation sampling (SURVEY section 8(f) rank 4): uniform points in a box, Philox4x32-10 counter-based
 // generator (Salmon et al., SC'11) keyed by `seed`, counter = (point index + offset, dimension group).  Replaces the
 // per-step numpy RNG + H2D copy of ContinuousNamedArrayDataset (ppsci/data/dataset/array_dataset.py:208-228) for boxes;

@@ -95,6 +95,56 @@ class PlanSpec(C.Structure):
     ]
 
 
+class DeepONetHeadSpec(C.Structure):
+    """Mirror of ``ppsci_deeponet_head_spec`` (include/ppsci_b200.h)."""
+
+    _fields_ = [
+        ("dtype", C.c_int32),
+        ("act", C.c_int32),
+        ("n_dir", C.c_int32),
+        ("dir_order", C.c_int32),
+        ("n_aux", C.c_int32),
+        ("n_reg", C.c_int32),
+        ("n_ops", C.c_int32),
+        ("prog", C.POINTER(C.c_int32)),
+        ("n_consts", C.c_int32),
+        ("consts", C.POINTER(C.c_double)),
+        ("n_res", C.c_int32),
+        ("res_reg", C.c_int32 * MAX_RES),
+        ("n_grad", C.c_int32),
+        ("grad_res", C.POINTER(C.c_int32)),
+        ("grad_in", C.POINTER(C.c_int32)),
+        ("grad_reg", C.POINTER(C.c_int32)),
+    ]
+
+
+class DeepONetJetArgs(C.Structure):
+    """Mirror of ``ppsci_deeponet_jet_args`` (include/ppsci_b200.h)."""
+
+    _fields_ = [
+        ("b", C.c_void_p),
+        ("ldb", C.c_int32),
+        ("t", C.c_void_p),
+        ("ldt", C.c_int32),
+        ("tplane", C.c_int64),
+        ("n", C.c_int64),
+        ("n_features", C.c_int32),
+        ("bias", C.c_void_p),
+        ("y_col", C.c_void_p),
+        ("aux_cols", C.c_void_p * MAX_IN),
+        ("x_off", C.c_int64),
+        ("label_cols", C.c_void_p * MAX_RES),
+        ("label_const", C.c_double * MAX_RES),
+        ("weight_cols", C.c_void_p * MAX_RES),
+        ("coef", C.c_double * MAX_RES),
+        ("residual_out", C.c_void_p * MAX_RES),
+        ("loss_acc", C.c_void_p),
+        ("bbar", C.c_void_p),
+        ("tbar", C.c_void_p),
+        ("dbias", C.c_void_p),
+    ]
+
+
 EXPORTED_SYMBOLS = (
     "ppsci_b200_plan_create",
     "ppsci_b200_plan_destroy",
@@ -109,6 +159,11 @@ EXPORTED_SYMBOLS = (
     "ppsci_b200_values_bwd_kept",
     "ppsci_b200_plan_chunk_points",
     "ppsci_b200_deeponet_head",
+    "ppsci_b200_jets_fwd_keep",
+    "ppsci_b200_jets_bwd_kept",
+    "ppsci_b200_deeponet_jet_head_create",
+    "ppsci_b200_deeponet_jet_head_run",
+    "ppsci_b200_deeponet_jet_head_destroy",
     "ppsci_b200_sample_uniform",
     "ppsci_b200_plan_last_launches",
     "ppsci_b200_plan_uses_tcgen05",
@@ -176,6 +231,16 @@ class Library:
         L.ppsci_b200_plan_chunk_points.restype = i32
         L.ppsci_b200_deeponet_head.argtypes = [i32, i32, vp, vp, vp, vp, vp, i64, i32, dbl, vp, vp, vp, vp, vp, vp]
         L.ppsci_b200_deeponet_head.restype = C.c_int
+        L.ppsci_b200_jets_fwd_keep.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i64, vp, vp, C.c_size_t, vp]
+        L.ppsci_b200_jets_fwd_keep.restype = C.c_int
+        L.ppsci_b200_jets_bwd_kept.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), i64, vp, vp, vp, C.c_size_t, vp]
+        L.ppsci_b200_jets_bwd_kept.restype = C.c_int
+        L.ppsci_b200_deeponet_jet_head_create.argtypes = [C.POINTER(DeepONetHeadSpec), C.POINTER(vp)]
+        L.ppsci_b200_deeponet_jet_head_create.restype = C.c_int
+        L.ppsci_b200_deeponet_jet_head_run.argtypes = [vp, C.POINTER(DeepONetJetArgs), vp]
+        L.ppsci_b200_deeponet_jet_head_run.restype = C.c_int
+        L.ppsci_b200_deeponet_jet_head_destroy.argtypes = [vp]
+        L.ppsci_b200_deeponet_jet_head_destroy.restype = None
         L.ppsci_b200_sample_uniform.argtypes = [i32, C.c_uint64, C.c_uint64, i64, i32, C.POINTER(dbl), C.POINTER(dbl), C.POINTER(vp), vp]
         L.ppsci_b200_sample_uniform.restype = C.c_int
         L.ppsci_b200_plan_last_launches.argtypes = [vp]

@@ -381,6 +381,41 @@ class ResidualPlan:
         self.two_phase_launches += self.last_launches
         self._kept = None
 
+    def jets_fwd_keep(self, inputs: Dict[str, torch.Tensor], params: torch.Tensor):
+        """Forward with the adjoint's stash kept (``ppsci_b200_jets_fwd_keep``, any number of jet channels, at most
+        ``chunk_points`` points); the output jets stay in this plan's workspace.  Returns (address of the output jets,
+        address of their adjoints, row pitch, plane stride): both [C][N][pitch] planes, the adjoints to be written by the
+        caller before ``jets_bwd_kept``."""
+        device = params.device
+        n, xs = self._inputs(inputs, device)
+        auxs = self._aux_tensors(inputs, self.compiled.aux_keys, n, device)
+        ws = self._workspace(n, device)
+        wptr, wbytes = self._aligned(ws)
+        self._kept = (xs, auxs, n)
+        rc = self.lib.lib.ppsci_b200_jets_fwd_keep(self.handle, self._ptr_array(xs, len(xs)), self._ptr_array(auxs, len(auxs)),
+                                                   n, params.data_ptr(), wptr, wbytes, self._stream(device))
+        self.lib.check(rc, "jets_fwd_keep")
+        offs = [int(self.lib.lib.ppsci_b200_plan_stash_offset(self.handle, n, code))
+                for code in (len(self.compiled.net.widths) - 1, 300)]
+        if min(offs) < 0:
+            raise RuntimeError("plan_stash_offset failed")
+        ld = (self.n_out + 3) // 4 * 4
+        return wptr + offs[0], wptr + offs[1], ld, n * ld
+
+    def jets_bwd_kept(self, params: torch.Tensor, grads: torch.Tensor):
+        """Adjoint of the most recent ``jets_fwd_keep`` from the output-jet adjoints the caller left in the workspace;
+        accumulates into ``grads``."""
+        xs, auxs, n = self._kept
+        device = params.device
+        if grads.dtype != params.dtype or grads.numel() != params.numel() or grads.device != device or not grads.is_contiguous():
+            raise ValueError("grads must match params in dtype/size/device and be contiguous")
+        ws = self._workspace(n, device)
+        wptr, wbytes = self._aligned(ws)
+        rc = self.lib.lib.ppsci_b200_jets_bwd_kept(self.handle, self._ptr_array(xs, len(xs)), self._ptr_array(auxs, len(auxs)),
+                                                   n, params.data_ptr(), grads.data_ptr(), wptr, wbytes, self._stream(device))
+        self.lib.check(rc, "jets_bwd_kept")
+        self._kept = None
+
     def forward(
         self,
         inputs: Dict[str, torch.Tensor],

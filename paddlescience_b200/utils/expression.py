@@ -305,12 +305,9 @@ class ExpressionSolver(nn.Module):
         if hasattr(model, "fused_train_forward"):  # models that combine several native networks (DeepONet)
             for i, cst_name in enumerate(constraint):
                 cst = constraint[cst_name]
-                extra = [k for k in cst.output_expr if k not in model.output_keys]
-                if extra:
-                    raise NotImplementedError(f"{type(model).__name__}: output expressions {extra} beyond the model outputs "
-                                              "are not supported on the fused training path")
-                weights = weight_dicts[i]
-                losses = model.fused_train_forward(cst.loss, input_dicts[i], label_dicts[i], weights)
+                extra = [k for k in input_dicts[i] if k not in model.input_keys]
+                losses = model.fused_train_forward(cst.loss, input_dicts[i], label_dicts[i], weight_dicts[i],
+                                                   cst.output_expr, extra)
                 losses_constraint[cst_name] = sum(losses.values())
                 for key, v in losses.items():
                     losses_all[key] = losses_all[key] + v if key in losses_all else v
@@ -385,6 +382,13 @@ class ExpressionSolver(nn.Module):
     def eval_forward(self, expr_dict, input_dict, model, validator, label_dict, weight_dict):
         """Forward for evaluation (expression.py:133-180): outputs + expressions + validator loss."""
         output_dict = model({k: input_dict[k] for k in model.input_keys})
+        if hasattr(model, "evaluate_expressions"):  # DeepONet: expressions over G(y) through its jet head
+            pending = {name: expr for name, expr in expr_dict.items()
+                       if not (name in output_dict and not isinstance(expr, (sp.Basic, symbolic.CompiledExpr)))}
+            if pending:
+                extra = [k for k in input_dict if k not in model.input_keys]
+                output_dict.update(model.evaluate_expressions(pending, input_dict, extra))
+            expr_dict = {}
         for name, expr in expr_dict.items():
             if name in output_dict and not isinstance(expr, (sp.Basic, symbolic.CompiledExpr)):
                 continue  # plain "lambda out: out['u']" style pass-through
