@@ -302,20 +302,26 @@ int ppsci_b200_jets_fwd_keep(ppsci_plan* plan, const void* const* x_cols, const 
 int ppsci_b200_jets_bwd_kept(ppsci_plan* plan, const void* const* x_cols, const void* const* aux_cols, int64_t n_points,
                              const void* params, void* grads, void* workspace, size_t workspace_bytes, void* stream);
 
-/* DeepONet residual head on Taylor jets — physics-informed DeepONet (Wang, Wang & Perdikaris 2021): residuals that
- * differentiate G(u)(y) = sum_i branch_i(u) act(trunk_i(y)) + b with respect to the trunk coordinate y, as the reference
- * trains through autograd (jacobian / hessian of G w.r.t. y).  The trunk net carries jets along y (one direction,
- * K = dir_order <= 4, C = 1 + K channels; n_dir = 0: values only), the branch net values only.  The residual program
- * is the one of ppsci_plan_spec for a network with n_out = 1 and n_in = 1: before it runs
- *   r[c] = G_c (channel c of G's jets, c < C),  r[C] = y,  r[C + 1 + a] = auxiliary column a.
- * Per pair the head forms G_c, runs the program, accumulates the per-slot MSE and writes the adjoints of both
- * sub-networks' outputs:  bbar_i = sum_c Gbar_c A_c[i],  tbar = adjoint of A = act(t) for the output-jet adjoints
- * b_i Gbar_c (all C channels),  dbias += Gbar_0. */
+/* Operator residual head on Taylor jets — physics-informed DeepONet (Wang, Wang & Perdikaris 2021) and HEDeepONets:
+ * residuals that differentiate  G_k(u)(y) = sum_{i in block k} f_i(u) act(trunk_i(y)) + b_k  with respect to the trunk
+ * inputs y, as the reference trains through autograd.  f_i = branch_i (DeepONet) or heat_i * cold_i (HEDeepONets, two
+ * branch factors); output k (k < n_out <= 3) reads the block of features k F .. (k+1) F - 1.  The trunk net carries the
+ * jets of the compiled layout (n_dir directions of orders dir_order[d], channels in direction order, C = 1 + sum of
+ * the orders; n_dir = 0: values only), the branch nets values only.  The residual program is the one of
+ * ppsci_plan_spec for a network with n_out outputs and n_in raw inputs: before it runs
+ *   r[c n_out + k] = G_{k,c} (channel c of output k's jets),  r[C n_out + j] = trunk input j,
+ *   r[C n_out + n_in + a] = auxiliary column a.
+ * Per pair the head forms G_{k,c}, runs the program, accumulates the per-slot MSE and writes the adjoints of all
+ * sub-networks' outputs: with S_i = sum_c Gbar_{k(i),c} A_c[i],  bbar_i = S_i (one branch) or b2_i S_i and
+ * b2bar_i = b_i S_i,  tbar = adjoint of A = act(t) for the output-jet adjoints f_i Gbar_{k(i),c} (all C channels),
+ * dbias[k] += Gbar_{k,0}.  C is at most 7. */
 typedef struct ppsci_deeponet_head_spec {
   int32_t dtype;
   int32_t act; /* trunk activation (PPSCI_ACT_*, none with a trainable parameter) */
-  int32_t n_dir; /* 0 or 1 */
-  int32_t dir_order; /* 1 .. PPSCI_MAX_ORDER when n_dir == 1 */
+  int32_t n_out; /* 1 .. 3 output blocks */
+  int32_t n_in;  /* 1 .. PPSCI_MAX_IN raw trunk inputs */
+  int32_t n_dir; /* 0 .. PPSCI_MAX_DIR */
+  int32_t dir_order[PPSCI_MAX_DIR]; /* 1 .. PPSCI_MAX_ORDER for d < n_dir */
   int32_t n_aux;
   int32_t n_reg;
   int32_t n_ops;
@@ -326,26 +332,29 @@ typedef struct ppsci_deeponet_head_spec {
   int32_t res_reg[PPSCI_MAX_RES];
   int32_t n_grad;
   const int32_t* grad_res; /* copied at create */
-  const int32_t* grad_in;  /* register index < C, sorted */
+  const int32_t* grad_in;  /* register index < C n_out, sorted */
   const int32_t* grad_reg;
 } ppsci_deeponet_head_spec;
 
-/* One call of the head over n pairs.  b: branch outputs [n][ldb]; t: trunk output jets [C][n][ldt], plane stride
- * tplane (both as jets_fwd_keep leaves them: they are read in place).  The columns y_col, aux_cols, label_cols,
+/* One call of the head over n pairs.  b: first branch's outputs [n][ldb]; b2: second branch's [n][ldb2] or NULL (one
+ * branch); t: trunk output jets [C][n][ldt], plane stride tplane (all as jets_fwd_keep leaves them: they are read in
+ * place); n_features = F, the width of one output block.  x_cols (n_in trunk input columns), aux_cols, label_cols,
  * weight_cols and residual_out are indexed from x_off.  coef[k] = loss weight of slot k (/ n_norm for "mean").
- * loss_acc: n_res device doubles, ACCUMULATED, or NULL.  bbar / tbar: the adjoints, same layouts as b / t (may be the
- * stash_offset 300 planes of the two plans), both or neither; NULL = forward only (residual_out / loss_acc).  dbias:
- * device scalar, accumulated, or NULL. */
+ * loss_acc: n_res device doubles, ACCUMULATED, or NULL.  bbar / b2bar / tbar: the adjoints, same layouts as b / b2 / t
+ * (may be the stash_offset 300 planes of the plans); bbar and tbar both or neither, b2bar exactly when b2 and bbar are
+ * given; NULL = forward only (residual_out / loss_acc).  dbias: n_out device values, accumulated, or NULL. */
 typedef struct ppsci_deeponet_jet_args {
   const void* b;
   int32_t ldb;
+  const void* b2;
+  int32_t ldb2;
   const void* t;
   int32_t ldt;
   int64_t tplane;
   int64_t n;
   int32_t n_features;
   const void* bias;
-  const void* y_col;
+  const void* x_cols[PPSCI_MAX_IN];
   const void* aux_cols[PPSCI_MAX_IN];
   int64_t x_off;
   const void* label_cols[PPSCI_MAX_RES];
@@ -355,6 +364,7 @@ typedef struct ppsci_deeponet_jet_args {
   void* residual_out[PPSCI_MAX_RES];
   double* loss_acc;
   void* bbar;
+  void* b2bar;
   void* tbar;
   void* dbias;
 } ppsci_deeponet_jet_args;

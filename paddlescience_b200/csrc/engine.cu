@@ -1339,7 +1339,7 @@ extern "C" int ppsci_b200_jets_bwd_kept(ppsci_plan* plan, const void* const* x_c
 struct ppsci_deeponet_head {
   ppsci_deeponet_head_spec spec;
   JetLayout J;
-  int kmax = 1;
+  int cb = 2;  // channel bound of the kernel instance
   int* d_prog = nullptr;
   double* d_consts = nullptr;
   int* d_grad_res = nullptr;
@@ -1363,14 +1363,21 @@ extern "C" int ppsci_b200_deeponet_jet_head_create(const ppsci_deeponet_head_spe
   if (s->dtype != PPSCI_F32 && s->dtype != PPSCI_F64) return fail("deeponet_jet_head_create: dtype must be f32 or f64");
   if (s->act < 0 || s->act > PPSCI_ACT_LAST) return fail("deeponet_jet_head_create: unknown activation");
   if (act_has_param(s->act)) return fail("deeponet_jet_head_create: activations with a trainable parameter are not offered here");
-  if (s->n_dir != 0 && s->n_dir != 1) return fail("deeponet_jet_head_create: n_dir must be 0 or 1 (the trunk coordinate)");
-  if (s->n_dir == 1 && (s->dir_order < 1 || s->dir_order > PPSCI_MAX_ORDER))
-    return fail("deeponet_jet_head_create: dir_order out of range");
+  if (s->n_out < 1 || s->n_out > DEEPONET_MAX_OUT) return fail("deeponet_jet_head_create: n_out must be 1 .. 3");
+  if (s->n_in < 1 || s->n_in > PPSCI_MAX_IN) return fail("deeponet_jet_head_create: n_in out of range");
+  if (s->n_dir < 0 || s->n_dir > PPSCI_MAX_DIR) return fail("deeponet_jet_head_create: n_dir out of range");
+  int C = 1;
+  for (int d = 0; d < s->n_dir; ++d) {
+    if (s->dir_order[d] < 1 || s->dir_order[d] > PPSCI_MAX_ORDER) return fail("deeponet_jet_head_create: dir_order out of range");
+    C += s->dir_order[d];
+  }
+  if (C > DEEPONET_MAX_CHANNELS)
+    return fail("deeponet_jet_head_create: " + std::to_string(C) + " jet channels; the largest head instance takes " +
+                std::to_string(DEEPONET_MAX_CHANNELS));
   if (s->n_aux < 0 || s->n_aux > PPSCI_MAX_IN) return fail("deeponet_jet_head_create: n_aux out of range");
   if (s->n_res < 1 || s->n_res > PPSCI_MAX_RES) return fail("deeponet_jet_head_create: n_res out of range");
-  const int C = 1 + (s->n_dir ? s->dir_order : 0);
-  if (check_program("deeponet_jet_head_create", C + 1 + s->n_aux, C, s->n_reg, s->n_ops, s->prog, s->n_consts, s->n_res,
-                    s->res_reg, s->n_grad, s->grad_res, s->grad_in, s->grad_reg))
+  if (check_program("deeponet_jet_head_create", C * s->n_out + s->n_in + s->n_aux, C * s->n_out, s->n_reg, s->n_ops, s->prog,
+                    s->n_consts, s->n_res, s->res_reg, s->n_grad, s->grad_res, s->grad_in, s->grad_reg))
     return 1;
   ppsci_deeponet_head* H = new ppsci_deeponet_head();
   H->spec = *s;
@@ -1380,9 +1387,11 @@ extern "C" int ppsci_b200_deeponet_jet_head_create(const ppsci_deeponet_head_spe
   memset(&H->J, 0, sizeof(H->J));
   H->J.C = C;
   H->J.n_dir = s->n_dir;
-  H->J.dir_order[0] = s->n_dir ? s->dir_order : 0;
-  H->J.dir_base[0] = 1;
-  H->kmax = C - 1 <= 1 ? 1 : (C - 1 == 2 ? 2 : 4);
+  for (int d = 0, base = 1; d < s->n_dir; base += s->dir_order[d], ++d) {
+    H->J.dir_order[d] = s->dir_order[d];
+    H->J.dir_base[d] = base;
+  }
+  H->cb = C <= 2 ? 2 : C <= 3 ? 3 : C <= 5 ? 5 : DEEPONET_MAX_CHANNELS;
   auto up = [&](const void* src, size_t bytes, void** dst) -> cudaError_t {
     cudaError_t e = cudaMalloc(dst, bytes ? bytes : 16);
     if (e != cudaSuccess) return e;
@@ -1406,11 +1415,15 @@ extern "C" int ppsci_b200_deeponet_jet_head_create(const ppsci_deeponet_head_spe
 extern "C" int ppsci_b200_deeponet_jet_head_run(const ppsci_deeponet_head* H, const ppsci_deeponet_jet_args* a, void* stream) {
   if (!H || !a) return fail("deeponet_jet_head_run: null argument");
   const ppsci_deeponet_head_spec& s = H->spec;
-  if (!a->b || !a->t || !a->y_col || a->n <= 0 || a->n_features <= 0 || a->x_off < 0)
-    return fail("deeponet_jet_head_run: bad arguments");
-  if (a->ldb < a->n_features || a->ldt < a->n_features || a->tplane < a->n * a->ldt)
-    return fail("deeponet_jet_head_run: row pitch or plane stride smaller than the features");
+  if (!a->b || !a->t || a->n <= 0 || a->n_features <= 0 || a->x_off < 0) return fail("deeponet_jet_head_run: bad arguments");
+  const long long width = (long long)s.n_out * a->n_features;
+  if (a->ldb < width || a->ldt < width || (a->b2 && a->ldb2 < width) || a->tplane < a->n * a->ldt)
+    return fail("deeponet_jet_head_run: row pitch or plane stride smaller than n_out * n_features");
   if ((a->bbar == nullptr) != (a->tbar == nullptr)) return fail("deeponet_jet_head_run: bbar and tbar must both be given or both be null");
+  if (a->b2bar && !a->b2) return fail("deeponet_jet_head_run: b2bar given without the second branch's features b2");
+  if (a->b2 && a->bbar && !a->b2bar) return fail("deeponet_jet_head_run: the adjoint of a two-branch head needs b2bar");
+  for (int j = 0; j < s.n_in; ++j)
+    if (!a->x_cols[j]) return fail("deeponet_jet_head_run: null trunk input column " + std::to_string(j));
   for (int i = 0; i < s.n_aux; ++i)
     if (!a->aux_cols[i]) return fail("deeponet_jet_head_run: null aux column " + std::to_string(i));
   return with_dtype(s.dtype, "deeponet_jet_head_run", [&](auto zero) {
@@ -1429,15 +1442,19 @@ extern "C" int ppsci_b200_deeponet_jet_head_run(const ppsci_deeponet_head* H, co
     h.P.grad_reg = H->d_grad_reg;
     h.J = H->J;
     h.act = s.act;
+    h.n_out = s.n_out;
+    h.n_in = s.n_in;
     h.b = (const T*)a->b;
     h.ldb = a->ldb;
+    h.b2 = (const T*)a->b2;
+    h.ldb2 = a->ldb2;
     h.t = (const T*)a->t;
     h.ldt = a->ldt;
     h.tplane = a->tplane;
     h.n = a->n;
     h.F = a->n_features;
     h.bias = (const T*)a->bias;
-    h.y_col = (const T*)a->y_col;
+    for (int j = 0; j < s.n_in; ++j) h.x_cols[j] = a->x_cols[j];
     for (int i = 0; i < s.n_aux; ++i) h.aux_cols[i] = a->aux_cols[i];
     h.n_aux = s.n_aux;
     h.x_off = a->x_off;
@@ -1450,12 +1467,15 @@ extern "C" int ppsci_b200_deeponet_jet_head_run(const ppsci_deeponet_head* H, co
     }
     h.loss_acc = a->loss_acc;
     h.bbar = (T*)a->bbar;
+    h.b2bar = (T*)a->b2bar;
     h.tbar = (T*)a->tbar;
     h.dbias = (T*)a->dbias;
     const long long warps = a->n < 132LL * 64 ? a->n : 132LL * 64;  // 8 warps per block
     const unsigned blocks = (unsigned)((warps + 7) / 8);
-    void (*k)(DeepONetJetArgs<T>) = H->kmax == 1 ? k_deeponet_jet_head<T, 1>
-                                   : H->kmax == 2 ? k_deeponet_jet_head<T, 2> : k_deeponet_jet_head<T, 4>;
+    void (*k)(DeepONetJetArgs<T>) = H->cb == 2   ? k_deeponet_jet_head<T, 2>
+                                   : H->cb == 3 ? k_deeponet_jet_head<T, 3>
+                                   : H->cb == 5 ? k_deeponet_jet_head<T, 5>
+                                                : k_deeponet_jet_head<T, DEEPONET_MAX_CHANNELS>;
     PPSCI_LAUNCH(k, dim3(blocks), dim3(256), 0, stream, h);
     CK(cudaGetLastError());
     return 0;

@@ -930,32 +930,42 @@ __global__ void __launch_bounds__(256) k_deeponet_head(const T* b, const T* t, c
   }
 }
 
-// DeepONet head on the trunk coordinate's Taylor jets (physics-informed DeepONet).  Per pair p, with A = act(t) the
-// activation jets of the trunk features along the one direction y (C = 1 + K channels):
-//   G_c = sum_i b_i A_c[i] (+ bias on c = 0);  residual program on r[c] = G_c, r[C] = y, r[C + 1 + a] = aux a (as k_head
-//   with n_out = 1);  per-slot MSE;  Gbar_c from the program's partials;
-//   bbar_i = sum_c Gbar_c A_c[i] (the branch does not depend on y),  tbar = jet_adj(act, t, ybar_c = b_i Gbar_c),
-//   dbias += Gbar_0.
-// One warp per pair: lanes stride the features, the C sums are butterfly-reduced so every lane holds them and runs the
-// (uniform) program itself.  b / bbar are [n][ldb], t / tbar [C][n][ldt] with plane stride tplane; the adjoint is written
-// only when bbar != NULL (then tbar too), padding columns F .. ld-1 of both get zeros.
+// Operator head on the trunk's Taylor jets (physics-informed DeepONet, HEDeepONets).  Per pair p, with A = act(t) the
+// activation jets of the trunk features (channels c < C of the plan's JetLayout, any compiled layout) and n_out output
+// blocks of F consecutive features (block k holds features kF .. (k+1)F - 1):
+//   f_i = b_i (one branch) or b_i b2_i (two branch factors);  G_{k,c} = sum_{i in k} f_i A_c[i] (+ bias[k] on c = 0);
+//   residual program on r[c n_out + k] = G_{k,c}, r[C n_out + j] = raw trunk input j, then the aux columns (the
+//   register order of k_head);  per-slot MSE;  Gbar_{k,c} from the program's partials;
+//   with S_i = sum_c Gbar_{k(i),c} A_c[i]:  bbar_i = S_i (one branch) or b2_i S_i, b2bar_i = b_i S_i;
+//   tbar = jet_adj(act, t, ybar_c = f_i Gbar_{k(i),c});  dbias[k] += Gbar_{k,0}.
+// One warp per pair: lanes stride the features of each block, the sums are butterfly-reduced so every lane holds them
+// and runs the (uniform) program itself.  b / bbar are [n][ldb], b2 / b2bar [n][ldb2], t / tbar [C][n][ldt] with plane
+// stride tplane; the adjoint is written only when bbar != NULL (then tbar, and b2bar with b2, too), padding columns
+// n_out F .. ld-1 of all of them get zeros.  CB bounds the channel count C; the Taylor order bound follows from it.
+constexpr int DEEPONET_MAX_OUT = 3;
+constexpr int DEEPONET_MAX_CHANNELS = 7;  // channel bound of the largest head instance
+
 template <typename T>
 struct DeepONetJetArgs {
   HeadProgram P;
   JetLayout J;
   int act;
+  int n_out;
+  int n_in;
   const T* b;
   int ldb;
+  const T* b2;
+  int ldb2;
   const T* t;
   int ldt;
   long long tplane;
   long long n;
   int F;
   const T* bias;
-  const T* y_col;
+  const void* x_cols[PPSCI_MAX_IN];
   const void* aux_cols[PPSCI_MAX_IN];
   int n_aux;
-  long long x_off;  // chunk offset into y_col / aux / label / weight / residual columns
+  long long x_off;  // chunk offset into x / aux / label / weight / residual columns
   const void* label_cols[PPSCI_MAX_RES];
   double label_const[PPSCI_MAX_RES];
   const void* weight_cols[PPSCI_MAX_RES];
@@ -963,45 +973,54 @@ struct DeepONetJetArgs {
   void* residual_out[PPSCI_MAX_RES];
   double* loss_acc;  // [n_res] fp64 accumulators or null
   T* bbar;
+  T* b2bar;
   T* tbar;
-  T* dbias;
+  T* dbias;  // [n_out] or null
 };
 
-template <typename T, int KMAX>
+template <typename T, int CB>
 __global__ void __launch_bounds__(256) k_deeponet_jet_head(DeepONetJetArgs<T> h) {
+  constexpr int KM = CB - 1 < 4 ? CB - 1 : 4;
+  constexpr int NO = DEEPONET_MAX_OUT;
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, wpb = blockDim.x >> 5;
-  const int C = h.J.C;
-  const T bias_v = h.bias ? h.bias[0] : T(0);
+  const int C = h.J.C, n_out = h.n_out;
   double part[PPSCI_MAX_RES];
   for (int k = 0; k < h.P.n_res; ++k) part[k] = 0.0;
-  T db_part = T(0);
+  T db_part[NO];
+#pragma unroll
+  for (int k = 0; k < NO; ++k) db_part[k] = T(0);
   T r[PPSCI_MAX_REG];
   for (long long p = (long long)blockIdx.x * wpb + wib; p < h.n; p += (long long)gridDim.x * wpb) {
     const T* bp = h.b + p * h.ldb;
+    const T* b2p = h.b2 ? h.b2 + p * h.ldb2 : nullptr;
     const T* tp = h.t + p * h.ldt;
-    T G[KMAX + 1];
+    T G[NO][CB];
 #pragma unroll
-    for (int c = 0; c <= KMAX; ++c) G[c] = T(0);
-    for (int i = lane; i < h.F; i += 32) {
-      T y0, s[6];
-      act_coef<T, KMAX>(h.act, tp[i], y0, s);
-      const T bi = bp[i];
-      G[0] += bi * y0;
-      jet_fwd<T, DynLay<KMAX>>(h.J, s, [&](int c) { return tp[(long long)c * h.tplane + i]; }, [&](int c, T v) {
+    for (int k = 0; k < NO; ++k) {
 #pragma unroll
-        for (int q = 1; q <= KMAX; ++q)
-          if (c == q) G[q] += bi * v;
-      });
+      for (int c = 0; c < CB; ++c) G[k][c] = T(0);
+      if (k >= n_out) continue;
+      for (int i = k * h.F + lane; i < (k + 1) * h.F; i += 32) {
+        T y0, s[6];
+        act_coef<T, KM>(h.act, tp[i], y0, s);
+        const T fi = b2p ? bp[i] * b2p[i] : bp[i];
+        G[k][0] += fi * y0;
+        jet_fwd<T, DynLay<KM>>(h.J, s, [&](int c) { return tp[(long long)c * h.tplane + i]; }, [&](int c, T v) {
+#pragma unroll
+          for (int q = 1; q < CB; ++q)
+            if (c == q) G[k][q] += fi * v;
+        });
+      }
+#pragma unroll
+      for (int c = 0; c < CB; ++c)
+        for (int o = 16; o > 0; o >>= 1) G[k][c] += __shfl_xor_sync(0xffffffffu, G[k][c], o);
+      if (h.bias) G[k][0] += h.bias[k];
+#pragma unroll
+      for (int c = 0; c < CB; ++c)
+        if (c < C) r[c * n_out + k] = G[k][c];
     }
-#pragma unroll
-    for (int c = 0; c <= KMAX; ++c)
-      for (int o = 16; o > 0; o >>= 1) G[c] += __shfl_xor_sync(0xffffffffu, G[c], o);
-    G[0] += bias_v;
-#pragma unroll
-    for (int c = 0; c <= KMAX; ++c)
-      if (c < C) r[c] = G[c];
-    r[C] = h.y_col[h.x_off + p];
-    for (int a = 0; a < h.n_aux; ++a) r[C + 1 + a] = reinterpret_cast<const T*>(h.aux_cols[a])[h.x_off + p];
+    for (int j = 0; j < h.n_in; ++j) r[C * n_out + j] = reinterpret_cast<const T*>(h.x_cols[j])[h.x_off + p];
+    for (int a = 0; a < h.n_aux; ++a) r[C * n_out + h.n_in + a] = reinterpret_cast<const T*>(h.aux_cols[a])[h.x_off + p];
     vm_run<T>(h.P, r);
     T rb[PPSCI_MAX_RES];
     for (int k = 0; k < h.P.n_res; ++k) {
@@ -1014,48 +1033,71 @@ __global__ void __launch_bounds__(256) k_deeponet_jet_head(DeepONetJetArgs<T> h)
       if (lane == 0) part[k] += (double)(w * e * e) * h.coef[k];
     }
     if (!h.bbar) continue;
-    T Gb[KMAX + 1];  // dLoss/dG_c; the grad list is sorted by grad_in (= c)
+    T Gb[NO][CB];  // dLoss/dG_{k,c}; each sums its grad-list terms in list order
 #pragma unroll
-    for (int c = 0; c <= KMAX; ++c) {
-      Gb[c] = T(0);
-      for (int g = 0; g < h.P.n_grad; ++g)
-        if (h.P.grad_in[g] == c) Gb[c] += rb[h.P.grad_res[g]] * r[h.P.grad_reg[g]];
+    for (int k = 0; k < NO; ++k)
+#pragma unroll
+      for (int c = 0; c < CB; ++c) Gb[k][c] = T(0);
+    for (int g = 0; g < h.P.n_grad; ++g) {
+      const int gi = h.P.grad_in[g];
+      const T v = rb[h.P.grad_res[g]] * r[h.P.grad_reg[g]];
+#pragma unroll
+      for (int k = 0; k < NO; ++k)
+#pragma unroll
+        for (int c = 0; c < CB; ++c)
+          if (gi == c * n_out + k) Gb[k][c] += v;
     }
-    if (lane == 0) db_part += Gb[0];
     T* bbp = h.bbar + p * h.ldb;
+    T* b2bp = h.b2bar ? h.b2bar + p * h.ldb2 : nullptr;
     T* tbp = h.tbar + p * h.ldt;
-    for (int i = lane; i < h.ldb || i < h.ldt; i += 32) {
-      if (i >= h.F) {  // padding of the row pitch: the sub-networks' adjoints read zeros there
-        if (i < h.ldb) bbp[i] = T(0);
-        if (i < h.ldt)
-          for (int c = 0; c < C; ++c) tbp[(long long)c * h.tplane + i] = T(0);
-        continue;
+#pragma unroll
+    for (int k = 0; k < NO; ++k) {
+      if (k >= n_out) continue;
+      if (lane == 0) db_part[k] += Gb[k][0];
+      for (int i = k * h.F + lane; i < (k + 1) * h.F; i += 32) {
+        T y0, s[6];
+        act_coef<T, KM + 1>(h.act, tp[i], y0, s);
+        const T bi = bp[i];
+        T acc = Gb[k][0] * y0;
+        auto z = [&](int c) { return tp[(long long)c * h.tplane + i]; };
+        jet_fwd<T, DynLay<KM>>(h.J, s, z, [&](int c, T v) {
+#pragma unroll
+          for (int q = 1; q < CB; ++q)
+            if (c == q) acc += Gb[k][q] * v;
+        });
+        T fi = bi;
+        if (b2p) {
+          const T ci = b2p[i];
+          fi = bi * ci;
+          b2bp[i] = bi * acc;
+          acc = ci * acc;
+        }
+        auto ybar = [&](int c) {
+          T g = Gb[k][0];
+#pragma unroll
+          for (int q = 1; q < CB; ++q)
+            if (c == q) g = Gb[k][q];
+          return fi * g;
+        };
+        tbp[i] = jet_adj<T, DynLay<KM>>(h.J, s, z, ybar, [&](int c, T v) { tbp[(long long)c * h.tplane + i] = v; });
+        bbp[i] = acc;
       }
-      T y0, s[6];
-      act_coef<T, KMAX + 1>(h.act, tp[i], y0, s);
-      const T bi = bp[i];
-      T bacc = Gb[0] * y0;
-      auto z = [&](int c) { return tp[(long long)c * h.tplane + i]; };
-      jet_fwd<T, DynLay<KMAX>>(h.J, s, z, [&](int c, T v) {
-#pragma unroll
-        for (int q = 1; q <= KMAX; ++q)
-          if (c == q) bacc += Gb[q] * v;
-      });
-      auto ybar = [&](int c) {
-        T g = Gb[0];
-#pragma unroll
-        for (int q = 1; q <= KMAX; ++q)
-          if (c == q) g = Gb[q];
-        return bi * g;
-      };
-      tbp[i] = jet_adj<T, DynLay<KMAX>>(h.J, s, z, ybar, [&](int c, T v) { tbp[(long long)c * h.tplane + i] = v; });
-      bbp[i] = bacc;
+    }
+    // padding of the row pitches: the sub-networks' adjoints read zeros there
+    for (int i = n_out * h.F + lane; i < h.ldb || i < h.ldt || (b2bp && i < h.ldb2); i += 32) {
+      if (i < h.ldb) bbp[i] = T(0);
+      if (b2bp && i < h.ldb2) b2bp[i] = T(0);
+      if (i < h.ldt)
+        for (int c = 0; c < C; ++c) tbp[(long long)c * h.tplane + i] = T(0);
     }
   }
   if (lane == 0) {
     if (h.loss_acc)
       for (int k = 0; k < h.P.n_res; ++k) atomicAdd(h.loss_acc + k, part[k]);
-    if (h.bbar && h.dbias) atomicAdd(h.dbias, db_part);
+    if (h.bbar && h.dbias)
+#pragma unroll
+      for (int k = 0; k < NO; ++k)
+        if (k < n_out) atomicAdd(h.dbias + k, db_part[k]);
   }
 }
 

@@ -101,8 +101,10 @@ class DeepONetHeadSpec(C.Structure):
     _fields_ = [
         ("dtype", C.c_int32),
         ("act", C.c_int32),
+        ("n_out", C.c_int32),
+        ("n_in", C.c_int32),
         ("n_dir", C.c_int32),
-        ("dir_order", C.c_int32),
+        ("dir_order", C.c_int32 * MAX_DIR),
         ("n_aux", C.c_int32),
         ("n_reg", C.c_int32),
         ("n_ops", C.c_int32),
@@ -124,13 +126,15 @@ class DeepONetJetArgs(C.Structure):
     _fields_ = [
         ("b", C.c_void_p),
         ("ldb", C.c_int32),
+        ("b2", C.c_void_p),
+        ("ldb2", C.c_int32),
         ("t", C.c_void_p),
         ("ldt", C.c_int32),
         ("tplane", C.c_int64),
         ("n", C.c_int64),
         ("n_features", C.c_int32),
         ("bias", C.c_void_p),
-        ("y_col", C.c_void_p),
+        ("x_cols", C.c_void_p * MAX_IN),
         ("aux_cols", C.c_void_p * MAX_IN),
         ("x_off", C.c_int64),
         ("label_cols", C.c_void_p * MAX_RES),
@@ -140,6 +144,7 @@ class DeepONetJetArgs(C.Structure):
         ("residual_out", C.c_void_p * MAX_RES),
         ("loss_acc", C.c_void_p),
         ("bbar", C.c_void_p),
+        ("b2bar", C.c_void_p),
         ("tbar", C.c_void_p),
         ("dbias", C.c_void_p),
     ]

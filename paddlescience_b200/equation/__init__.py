@@ -1,6 +1,6 @@
-from .pde import PDE, AllenCahn, Biharmonic, Helmholtz, Laplace, NavierStokes, Poisson, Vibration
+from .pde import PDE, AllenCahn, Biharmonic, HeatExchanger, Helmholtz, Laplace, NavierStokes, Poisson, Vibration
 
-__all__ = ["PDE", "AllenCahn", "Biharmonic", "Helmholtz", "Laplace", "NavierStokes", "Poisson", "Vibration", "build_equation"]
+__all__ = ["PDE", "AllenCahn", "Biharmonic", "HeatExchanger", "Helmholtz", "Laplace", "NavierStokes", "Poisson", "Vibration", "build_equation"]
 
 
 def build_equation(cfg):

@@ -382,12 +382,10 @@ class ExpressionSolver(nn.Module):
     def eval_forward(self, expr_dict, input_dict, model, validator, label_dict, weight_dict):
         """Forward for evaluation (expression.py:133-180): outputs + expressions + validator loss."""
         output_dict = model({k: input_dict[k] for k in model.input_keys})
-        if hasattr(model, "evaluate_expressions"):  # DeepONet: expressions over G(y) through its jet head
-            pending = {name: expr for name, expr in expr_dict.items()
-                       if not (name in output_dict and not isinstance(expr, (sp.Basic, symbolic.CompiledExpr)))}
-            if pending:
+        if hasattr(model, "evaluate_expressions"):  # operator networks: expressions through their jet head
+            if expr_dict:  # a pass-through is an expression that traces to exactly its output, whatever its form
                 extra = [k for k in input_dict if k not in model.input_keys]
-                output_dict.update(model.evaluate_expressions(pending, input_dict, extra))
+                output_dict.update(model.evaluate_expressions(expr_dict, input_dict, extra, outputs=output_dict))
             expr_dict = {}
         for name, expr in expr_dict.items():
             if name in output_dict and not isinstance(expr, (sp.Basic, symbolic.CompiledExpr)):
