@@ -417,12 +417,12 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_layer(WgArgs g) {
 //
 // CTA (fan-in block of 128 rows, column block of BN <= 128 columns, range of chunks): warpgroup i owns fan-in rows
 // 64 i .. 64 i + 63 and issues  A_hi B_hi -> exact accumulator,  A_lo B_hi + A_hi B_lo -> cross accumulator  per K step
-// (the 3xTF32 scheme of k_wg_layer, with the exact-product term in an accumulator of its own).  While the MMAs of chunk j
-// run, the Zbar_l values of chunk j + 1 are loaded into registers and written to the other B stage, and its Z_{l-1}
-// values are copied into per-thread shared-memory slots by cp.async (they would not fit in registers beside the two
-// accumulators and the in-flight A fragments); the jets are computed once those MMAs have retired.  Every dw_flush(C)
-// chunks each thread adds its accumulators to partial sums of its own in shared memory (fp32, round to nearest) and
-// restarts them at zero.  The CTA adds partial sums and accumulators to dW_l once, with atomicAdd; the CTAs of fan-in
+// (the 3xTF32 scheme of k_wg_layer, with the exact-product term in an accumulator of its own).  The Zbar_l values of
+// chunk j + 1 are loaded into registers right after chunk j's barrier, before its MMAs are issued, and written to the
+// other B stage while those MMAs run; its Z_{l-1} values are copied into per-thread shared-memory slots by cp.async
+// (they would not fit in registers beside the two accumulators and the in-flight A fragments); the jets are computed
+// once those MMAs have retired.  Every dw_flush(C) chunks each thread adds its accumulators to partial sums of its own
+// in shared memory (fp32, round to nearest) and restarts them at zero.  The CTA adds partial sums and accumulators to dW_l once, with atomicAdd; the CTAs of fan-in
 // block 0 also add their columns' channel-0 sums (summed in shared memory) to db_l.
 //
 // Why the periodic flush: the tensor cores do not round each accumulation to nearest, so the error of a wgmma
@@ -628,6 +628,9 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_dw(WgDwArgs g) {
     if (ch + 1 < ch_end) load_a(ch + 1);
     fence_proxy_async();
     __syncthreads();  // this chunk's B stage is complete
+    // the next chunk's Zbar_l loads go out before this chunk's MMAs: issued after them, their latency was measured to add
+    // to the MMAs' time instead of hiding under it (DESIGN.md 4.1).  zb is free: this chunk's values are in the stage
+    if (ch + 1 < ch_end) load_b(ch + 1);
     // K step s: a0 / a1 = group 2 s (rows krow / krow + 8), a2 / a3 = group 2 s + 1; group gi = channel gi % C of quad
     // gi / C
 #pragma unroll
@@ -662,7 +665,6 @@ __global__ void __launch_bounds__(THREADS, 1) k_wg_dw(WgDwArgs g) {
       }
     }
     wgmma_commit();
-    if (ch + 1 < ch_end) load_b(ch + 1);
   }
   wgmma_wait<0>();
 #pragma unroll
