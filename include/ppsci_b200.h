@@ -85,6 +85,9 @@ enum {
   PPSCI_OP_SINH = 20,
   PPSCI_OP_COSH = 21,
   PPSCI_OP_HEAVISIDE = 22,
+  PPSCI_OP_EQ = 23,     /* dst = r[a] == r[b] ? 1 : 0 */
+  PPSCI_OP_SELECT = 24, /* dst = r[dst] != 0 ? r[a] : r[b]  (accumulate form: the condition sits in dst); a true
+                         * select, so a NaN or Inf of the untaken operand never reaches dst */
 };
 
 /* MSELoss reduction — ppsci/loss/mse.py:82-106 */
@@ -304,16 +307,16 @@ int ppsci_b200_jets_bwd_kept(ppsci_plan* plan, const void* const* x_cols, const 
 
 /* Operator residual head on Taylor jets — physics-informed DeepONet (Wang, Wang & Perdikaris 2021) and HEDeepONets:
  * residuals that differentiate  G_k(u)(y) = sum_{i in block k} f_i(u) act(trunk_i(y)) + b_k  with respect to the trunk
- * inputs y, as the reference trains through autograd.  f_i = branch_i (DeepONet) or heat_i * cold_i (HEDeepONets, two
- * branch factors); output k (k < n_out <= 3) reads the block of features k F .. (k+1) F - 1.  The trunk net carries the
+ * inputs y, as the reference trains through autograd.  f_i = branch_i (DeepONet), heat_i * cold_i (HEDeepONets, two
+ * branch factors) or u_i * bc_i * bctype_i (ChipDeepONets, three branch factors); output k (k < n_out <= 3) reads the block of features k F .. (k+1) F - 1.  The trunk net carries the
  * jets of the compiled layout (n_dir directions of orders dir_order[d], channels in direction order, C = 1 + sum of
  * the orders; n_dir = 0: values only), the branch nets values only.  The residual program is the one of
  * ppsci_plan_spec for a network with n_out outputs and n_in raw inputs: before it runs
  *   r[c n_out + k] = G_{k,c} (channel c of output k's jets),  r[C n_out + j] = trunk input j,
  *   r[C n_out + n_in + a] = auxiliary column a.
  * Per pair the head forms G_{k,c}, runs the program, accumulates the per-slot MSE and writes the adjoints of all
- * sub-networks' outputs: with S_i = sum_c Gbar_{k(i),c} A_c[i],  bbar_i = S_i (one branch) or b2_i S_i and
- * b2bar_i = b_i S_i,  tbar = adjoint of A = act(t) for the output-jet adjoints f_i Gbar_{k(i),c} (all C channels),
+ * sub-networks' outputs: with S_i = sum_c Gbar_{k(i),c} A_c[i],  bbar_i = S_i (one branch), b2_i S_i and
+ * b2bar_i = b_i S_i (two), or b2_i b3_i S_i, b2bar_i = b_i b3_i S_i and b3bar_i = b_i b2_i S_i (three),  tbar = adjoint of A = act(t) for the output-jet adjoints f_i Gbar_{k(i),c} (all C channels),
  * dbias[k] += Gbar_{k,0}.  C is at most 7. */
 typedef struct ppsci_deeponet_head_spec {
   int32_t dtype;
@@ -337,12 +340,12 @@ typedef struct ppsci_deeponet_head_spec {
 } ppsci_deeponet_head_spec;
 
 /* One call of the head over n pairs.  b: first branch's outputs [n][ldb]; b2: second branch's [n][ldb2] or NULL (one
- * branch); t: trunk output jets [C][n][ldt], plane stride tplane (all as jets_fwd_keep leaves them: they are read in
+ * branch); b3: third branch's [n][ldb3] or NULL, only together with b2; t: trunk output jets [C][n][ldt], plane stride tplane (all as jets_fwd_keep leaves them: they are read in
  * place); n_features = F, the width of one output block.  x_cols (n_in trunk input columns), aux_cols, label_cols,
  * weight_cols and residual_out are indexed from x_off.  coef[k] = loss weight of slot k (/ n_norm for "mean").
  * loss_acc: n_res device doubles, ACCUMULATED, or NULL.  bbar / b2bar / tbar: the adjoints, same layouts as b / b2 / t
  * (may be the stash_offset 300 planes of the plans); bbar and tbar both or neither, b2bar exactly when b2 and bbar are
- * given; NULL = forward only (residual_out / loss_acc).  dbias: n_out device values, accumulated, or NULL. */
+ * given, b3bar exactly when b3 and bbar are given; NULL = forward only (residual_out / loss_acc).  dbias: n_out device values, accumulated, or NULL. */
 typedef struct ppsci_deeponet_jet_args {
   const void* b;
   int32_t ldb;
@@ -367,6 +370,9 @@ typedef struct ppsci_deeponet_jet_args {
   void* b2bar;
   void* tbar;
   void* dbias;
+  const void* b3; /* appended: the fields above keep their offsets */
+  int32_t ldb3;
+  void* b3bar;
 } ppsci_deeponet_jet_args;
 
 typedef struct ppsci_deeponet_head ppsci_deeponet_head;

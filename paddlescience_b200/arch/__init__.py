@@ -2,9 +2,10 @@ from .base import Arch
 from .mlp import MLP, ModifiedMLP, PirateNet
 from .deeponet import DeepONet
 from .he_deeponets import HEDeepONets
+from .chip_deeponets import ChipDeepONets
 from .activation import get_activation
 
-__all__ = ["Arch", "MLP", "ModifiedMLP", "PirateNet", "DeepONet", "HEDeepONets", "get_activation", "build_model"]
+__all__ = ["Arch", "MLP", "ModifiedMLP", "PirateNet", "DeepONet", "HEDeepONets", "ChipDeepONets", "get_activation", "build_model"]
 
 
 def build_model(cfg):

@@ -15,7 +15,7 @@ from __future__ import annotations
 import ctypes as C
 import math
 from collections import OrderedDict
-from typing import Dict, List, Sequence, Tuple, Union
+from typing import Dict, List, NamedTuple, Sequence, Tuple, Union
 
 import sympy as sp
 import torch
@@ -35,33 +35,47 @@ _TORCH_ACT = {
 }
 
 
+class SubNet(NamedTuple):
+    """The reference's ``mlp.MLP`` settings of one sub-network; ``prefix`` names its constructor arguments
+    (``{prefix}_weight_norm``, ...)."""
+
+    prefix: str
+    num_layers: object
+    hidden_size: object
+    skip_connection: bool
+    activation: str
+    weight_norm: bool
+
+
 class BranchTrunkArch(base.Arch):
     """Operators  G_k = sum_{i in block k} f_i * act(trunk(y))_i + b_k  (k < n_out, block k = features kF .. (k+1)F - 1)
-    with f = branch(u) (DeepONet) or the product of several branch nets' features (HEDeepONets, he_deeponets.py:151-193).
+    with f = branch(u) (DeepONet) or the product of several branch nets' features (HEDeepONets, he_deeponets.py:151-193;
+    ChipDeepONets, chip_deeponets.py:175-199).
 
     One flat parameter buffer  [branch 1 | ... | trunk | b]  (each sub-network starts at a multiple of 4), then the
     weight-norm gains of every sub-network in the same order.  Physics-informed constraints and expression evaluation
     run through one native head (``k_deeponet_jet_head``): the trunk carries the jets of the compiled residual set, the
     branch nets run values only."""
 
-    def _setup(self, branches: Sequence[Tuple[str, Tuple[str, ...], int]], trunk: Tuple[str, Tuple[str, ...]],
-               output_keys: Tuple[str, ...], num_features: int, branch_num_layers, trunk_num_layers, branch_hidden_size,
-               trunk_hidden_size, branch_skip_connection: bool, trunk_skip_connection: bool, branch_activation: str,
-               trunk_activation: str, branch_weight_norm: bool, trunk_weight_norm: bool, use_bias: bool, dtype: torch.dtype):
-        """``branches``: (reference name, input keys, input width) of every branch net; ``trunk``: (reference name,
-        input keys) of the trunk net."""
+    def _setup(self, branches: Sequence[Tuple[str, Tuple[str, ...], int, SubNet]], trunk: Tuple[str, Tuple[str, ...], SubNet],
+               output_keys: Tuple[str, ...], num_features: int, use_bias: bool, dtype: torch.dtype):
+        """``branches``: (reference name, input keys, input width, settings) of every branch net; ``trunk``: (reference
+        name, input keys, settings) of the trunk net."""
         cls = type(self).__name__
-        for wn, sk, name in ((branch_weight_norm, branch_skip_connection, "branch"), (trunk_weight_norm, trunk_skip_connection, "trunk")):
-            if wn and sk:  # the reference picks WeightNormLinear first and then applies the skip to it (mlp.py:238-296)
-                raise NotImplementedError(f"{cls}({name}_weight_norm=True, {name}_skip_connection=True) is not supported yet")
+        for sub in [b[3] for b in branches] + [trunk[2]]:
+            if sub.weight_norm and sub.skip_connection:
+                # the reference picks WeightNormLinear first and then applies the skip to it (mlp.py:238-296)
+                p = sub.prefix
+                raise NotImplementedError(f"{cls}({p}_weight_norm=True, {p}_skip_connection=True) is not supported yet")
         self.output_keys = tuple(output_keys)
         self.num_features, self.use_bias = int(num_features), bool(use_bias)
-        self._branch_keys = [tuple(keys) for _, keys, _ in branches]
-        self._branch_locs = [int(loc) for _, _, loc in branches]
+        self._branch_keys = [tuple(keys) for _, keys, _, _ in branches]
+        self._branch_locs = [int(loc) for _, _, loc, _ in branches]
         self._trunk_keys = tuple(trunk[1])
-        self.branch_activation = act_mod.get_activation(branch_activation)
-        self.trunk_activation = act_mod.get_activation(trunk_activation)
-        for a in (self.branch_activation, self.trunk_activation):
+        branch_acts = [act_mod.get_activation(sub.activation) for _, _, _, sub in branches]
+        self.branch_activation = branch_acts[0]
+        self.trunk_activation = act_mod.get_activation(trunk[2].activation)
+        for a in branch_acts + [self.trunk_activation]:
             if a == "stan":
                 raise NotImplementedError(f"{cls}(*_activation='stan'): activations with a trainable parameter are "
                                           "supported by arch.MLP only")
@@ -71,14 +85,14 @@ class BranchTrunkArch(base.Arch):
         width = n_out * self.num_features
         feats = tuple(f"f{i}" for i in range(width))
         nets, lo = [], 0
-        for (_, keys, loc) in branches:
-            bw = [int(loc)] + hidden_sizes(branch_num_layers, branch_hidden_size) + [width]
-            nets.append((NetSpec((keys[0],), feats, [], [], [], bw, self.branch_activation, dense_in=True),
-                         branch_weight_norm, branch_skip_connection))
+        for (_, keys, loc, sub), act in zip(branches, branch_acts):
+            bw = [int(loc)] + hidden_sizes(sub.num_layers, sub.hidden_size) + [width]
+            nets.append((NetSpec((keys[0],), feats, [], [], [], bw, act, dense_in=True), sub.weight_norm, sub.skip_connection))
         n_in = len(self._trunk_keys)
-        tw = [n_in] + hidden_sizes(trunk_num_layers, trunk_hidden_size) + [width]
+        ts = trunk[2]
+        tw = [n_in] + hidden_sizes(ts.num_layers, ts.hidden_size) + [width]
         nets.append((NetSpec(self._trunk_keys, feats, list(range(n_in)), [0] * n_in, [0.0] * n_in, tw, self.trunk_activation),
-                     trunk_weight_norm, trunk_skip_connection))
+                     ts.weight_norm, ts.skip_connection))
         los = []
         for net, _, _ in nets:
             los.append(lo)
@@ -98,7 +112,7 @@ class BranchTrunkArch(base.Arch):
             self._subnets.append(Reparam(shapes, lo, n, g_off, wn, doubled))
             if wn or doubled:
                 self._staged.append(self._subnets[-1])
-        self._sub_names = [name for name, _, _ in branches] + [trunk[0]]
+        self._sub_names = [b[0] for b in branches] + [trunk[0]]
         self._eff = self._eff_grad = None  # staging buffers laid out like flat, allocated on first use
         self.flat = nn.Parameter(torch.zeros(off, dtype=dtype))
         self.reset_parameters()
@@ -343,13 +357,15 @@ class BranchTrunkArch(base.Arch):
             sl = slice(s0, min(n, s0 + chunk))
             kept = [pb.jets_fwd_keep({self._branch_keys[j][0]: us[j][sl]}, params[j]) for j, pb in enumerate(pbs)]
             a.b, bbar, a.ldb, _ = kept[0]
-            b2bar = None
+            b2bar = b3bar = None
             if len(kept) > 1:
                 a.b2, b2bar, a.ldb2, _ = kept[1]
+            if len(kept) > 2:
+                a.b3, b3bar, a.ldb3, _ = kept[2]
             a.t, tbar, a.ldt, a.tplane = pt.jets_fwd_keep({k: x[sl] for k, x in zip(self._trunk_keys, xs)}, params[-1])
             a.n = sl.stop - s0
             a.x_off = s0
-            a.bbar, a.b2bar, a.tbar = (bbar, b2bar, tbar) if train else (None, None, None)
+            a.bbar, a.b2bar, a.b3bar, a.tbar = (bbar, b2bar, b3bar, tbar) if train else (None, None, None, None)
             lib.check(lib.lib.ppsci_b200_deeponet_jet_head_run(head.handle, C.byref(a), stream), "deeponet_jet_head_run")
             if train:
                 for pb, g, p in zip(pbs + (pt,), grads, params):
@@ -442,9 +458,11 @@ class DeepONet(BranchTrunkArch):
         self.u_key, self.y_key = u_key, y_key
         self.input_keys = (u_key, y_key)
         self.num_loc = int(num_loc)
-        self._setup([("branch_net", (u_key,), num_loc)], ("trunk_net", (y_key,)), (G_key,), num_features, branch_num_layers,
-                    trunk_num_layers, branch_hidden_size, trunk_hidden_size, branch_skip_connection, trunk_skip_connection,
-                    branch_activation, trunk_activation, branch_weight_norm, trunk_weight_norm, use_bias, dtype)
+        branch = SubNet("branch", branch_num_layers, branch_hidden_size, branch_skip_connection, branch_activation,
+                        branch_weight_norm)
+        trunk = SubNet("trunk", trunk_num_layers, trunk_hidden_size, trunk_skip_connection, trunk_activation, trunk_weight_norm)
+        self._setup([("branch_net", (u_key,), num_loc, branch)], ("trunk_net", (y_key,), trunk), (G_key,), num_features,
+                    use_bias, dtype)
         self._branch, self._trunk = self._nets
         self._rb, self._rt = self._subnets
 

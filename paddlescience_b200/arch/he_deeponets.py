@@ -13,7 +13,7 @@ from typing import Dict, Tuple, Union
 
 import torch
 
-from .deeponet import BranchTrunkArch
+from .deeponet import BranchTrunkArch, SubNet
 
 
 class HEDeepONets(BranchTrunkArch):
@@ -52,10 +52,11 @@ class HEDeepONets(BranchTrunkArch):
         self.heat_input_keys, self.cold_input_keys = tuple(heat_input_keys), tuple(cold_input_keys)
         self.trunk_input_keys = tuple(trunk_input_keys)
         self.input_keys = self.trunk_input_keys + self.heat_input_keys + self.cold_input_keys
-        self._setup([("heat_net", self.heat_input_keys, heat_num_loc), ("cold_net", self.cold_input_keys, cold_num_loc)],
-                    ("trunk_net", self.trunk_input_keys), output_keys, num_features, branch_num_layers, trunk_num_layers,
-                    branch_hidden_size, trunk_hidden_size, branch_skip_connection, trunk_skip_connection,
-                    branch_activation, trunk_activation, branch_weight_norm, trunk_weight_norm, use_bias, dtype)
+        branch = SubNet("branch", branch_num_layers, branch_hidden_size, branch_skip_connection, branch_activation,
+                        branch_weight_norm)
+        trunk = SubNet("trunk", trunk_num_layers, trunk_hidden_size, trunk_skip_connection, trunk_activation, trunk_weight_norm)
+        self._setup([("heat_net", self.heat_input_keys, heat_num_loc, branch), ("cold_net", self.cold_input_keys, cold_num_loc, branch)],
+                    ("trunk_net", self.trunk_input_keys, trunk), output_keys, num_features, use_bias, dtype)
 
     def fused_train_forward(self, loss_fn, input_dict, label_dict, weight_dict, output_expr=None,
                             extra_keys=()) -> Dict[str, torch.Tensor]:

@@ -53,6 +53,15 @@ class SymTensor:
     def __pow__(self, o): return SymTensor(self.expr ** self._unwrap(o))
     def __rpow__(self, o): return SymTensor(self._unwrap(o) ** self.expr)
     def __neg__(self): return SymTensor(-self.expr)
+    # comparisons are conditions of torch.where; the residual compiler takes equalities only and names that form for
+    # the others
+    def __eq__(self, o): return SymTensor(sp.Eq(self.expr, self._unwrap(o)))
+    def __ne__(self, o): return SymTensor(sp.Ne(self.expr, self._unwrap(o)))
+    def __lt__(self, o): return SymTensor(sp.Lt(self.expr, self._unwrap(o)))
+    def __le__(self, o): return SymTensor(sp.Le(self.expr, self._unwrap(o)))
+    def __gt__(self, o): return SymTensor(sp.Gt(self.expr, self._unwrap(o)))
+    def __ge__(self, o): return SymTensor(sp.Ge(self.expr, self._unwrap(o)))
+    __hash__ = object.__hash__
     def __pos__(self): return self
     def __repr__(self): return f"SymTensor({self.expr})"
 
@@ -87,6 +96,9 @@ class SymTensor:
             return SymTensor(sp.Max(cls._unwrap(args[0]), cls._unwrap(args[1])))
         if func in (torch.minimum,):
             return SymTensor(sp.Min(cls._unwrap(args[0]), cls._unwrap(args[1])))
+        if func is torch.where and len(args) == 3 and not kwargs:
+            cond, a, b = (cls._unwrap(t) for t in args)
+            return SymTensor(sp.Piecewise((a, cond), (b, True)))
         raise NotImplementedError(
             f"torch function {getattr(func, '__name__', func)} cannot be traced into a residual program")
 

@@ -195,7 +195,7 @@ static int op_arity(int op) {
     case PPSCI_OP_SIGN: case PPSCI_OP_SINH: case PPSCI_OP_COSH: case PPSCI_OP_HEAVISIDE:
       return 1;
     case PPSCI_OP_ADD: case PPSCI_OP_SUB: case PPSCI_OP_MUL: case PPSCI_OP_DIV: case PPSCI_OP_POW:
-    case PPSCI_OP_MAX: case PPSCI_OP_MIN: case PPSCI_OP_FMA:
+    case PPSCI_OP_MAX: case PPSCI_OP_MIN: case PPSCI_OP_FMA: case PPSCI_OP_EQ: case PPSCI_OP_SELECT:
       return 2;
     default: return -1;
   }
@@ -1417,11 +1417,15 @@ extern "C" int ppsci_b200_deeponet_jet_head_run(const ppsci_deeponet_head* H, co
   const ppsci_deeponet_head_spec& s = H->spec;
   if (!a->b || !a->t || a->n <= 0 || a->n_features <= 0 || a->x_off < 0) return fail("deeponet_jet_head_run: bad arguments");
   const long long width = (long long)s.n_out * a->n_features;
-  if (a->ldb < width || a->ldt < width || (a->b2 && a->ldb2 < width) || a->tplane < a->n * a->ldt)
+  if (a->ldb < width || a->ldt < width || (a->b2 && a->ldb2 < width) || (a->b3 && a->ldb3 < width) ||
+      a->tplane < a->n * a->ldt)
     return fail("deeponet_jet_head_run: row pitch or plane stride smaller than n_out * n_features");
   if ((a->bbar == nullptr) != (a->tbar == nullptr)) return fail("deeponet_jet_head_run: bbar and tbar must both be given or both be null");
   if (a->b2bar && !a->b2) return fail("deeponet_jet_head_run: b2bar given without the second branch's features b2");
   if (a->b2 && a->bbar && !a->b2bar) return fail("deeponet_jet_head_run: the adjoint of a two-branch head needs b2bar");
+  if (a->b3 && !a->b2) return fail("deeponet_jet_head_run: a third branch factor b3 needs the second one, b2");
+  if ((a->b3bar != nullptr) != (a->b3 != nullptr && a->bbar != nullptr))
+    return fail("deeponet_jet_head_run: b3bar must be given exactly when b3 and bbar are");
   for (int j = 0; j < s.n_in; ++j)
     if (!a->x_cols[j]) return fail("deeponet_jet_head_run: null trunk input column " + std::to_string(j));
   for (int i = 0; i < s.n_aux; ++i)
@@ -1470,12 +1474,17 @@ extern "C" int ppsci_b200_deeponet_jet_head_run(const ppsci_deeponet_head* H, co
     h.b2bar = (T*)a->b2bar;
     h.tbar = (T*)a->tbar;
     h.dbias = (T*)a->dbias;
+    h.b3 = (const T*)a->b3;
+    h.ldb3 = a->ldb3;
+    h.b3bar = (T*)a->b3bar;
     const long long warps = a->n < 132LL * 64 ? a->n : 132LL * 64;  // 8 warps per block
     const unsigned blocks = (unsigned)((warps + 7) / 8);
-    void (*k)(DeepONetJetArgs<T>) = H->cb == 2   ? k_deeponet_jet_head<T, 2>
-                                   : H->cb == 3 ? k_deeponet_jet_head<T, 3>
-                                   : H->cb == 5 ? k_deeponet_jet_head<T, 5>
-                                                : k_deeponet_jet_head<T, DEEPONET_MAX_CHANNELS>;
+    using K = void (*)(DeepONetJetArgs<T>);
+    const K ks[2][4] = {{k_deeponet_jet_head<T, 2, false>, k_deeponet_jet_head<T, 3, false>, k_deeponet_jet_head<T, 5, false>,
+                         k_deeponet_jet_head<T, DEEPONET_MAX_CHANNELS, false>},
+                        {k_deeponet_jet_head<T, 2, true>, k_deeponet_jet_head<T, 3, true>, k_deeponet_jet_head<T, 5, true>,
+                         k_deeponet_jet_head<T, DEEPONET_MAX_CHANNELS, true>}};
+    const K k = ks[a->b3 != nullptr][H->cb == 2 ? 0 : H->cb == 3 ? 1 : H->cb == 5 ? 2 : 3];
     PPSCI_LAUNCH(k, dim3(blocks), dim3(256), 0, stream, h);
     CK(cudaGetLastError());
     return 0;

@@ -799,6 +799,8 @@ __device__ __forceinline__ void vm_run(const HeadProgram& P, T* r) {
       case PPSCI_OP_SINH: v = T(sinh((double)r[a])); break;
       case PPSCI_OP_COSH: v = T(cosh((double)r[a])); break;
       case PPSCI_OP_HEAVISIDE: v = r[a] > T(0) ? T(1) : (r[a] < T(0) ? T(0) : T(0.5)); break;
+      case PPSCI_OP_EQ: v = r[a] == r[b] ? T(1) : T(0); break;
+      case PPSCI_OP_SELECT: v = r[dst] != T(0) ? r[a] : r[b]; break;  // never a blend: the untaken side may be NaN
       default: v = T(0); break;
     }
     r[dst] = v;
@@ -933,15 +935,19 @@ __global__ void __launch_bounds__(256) k_deeponet_head(const T* b, const T* t, c
 // Operator head on the trunk's Taylor jets (physics-informed DeepONet, HEDeepONets).  Per pair p, with A = act(t) the
 // activation jets of the trunk features (channels c < C of the plan's JetLayout, any compiled layout) and n_out output
 // blocks of F consecutive features (block k holds features kF .. (k+1)F - 1):
-//   f_i = b_i (one branch) or b_i b2_i (two branch factors);  G_{k,c} = sum_{i in k} f_i A_c[i] (+ bias[k] on c = 0);
+//   f_i = b_i (one branch), b_i b2_i (two branch factors) or b_i b2_i b3_i (three);  G_{k,c} = sum_{i in k} f_i A_c[i] (+ bias[k] on c = 0);
 //   residual program on r[c n_out + k] = G_{k,c}, r[C n_out + j] = raw trunk input j, then the aux columns (the
 //   register order of k_head);  per-slot MSE;  Gbar_{k,c} from the program's partials;
-//   with S_i = sum_c Gbar_{k(i),c} A_c[i]:  bbar_i = S_i (one branch) or b2_i S_i, b2bar_i = b_i S_i;
+//   with S_i = sum_c Gbar_{k(i),c} A_c[i]:  bbar_i = S_i (one branch) or b2_i S_i, b2bar_i = b_i S_i (two), or
+//   bbar_i = b2_i b3_i S_i, b2bar_i = b_i b3_i S_i, b3bar_i = b_i b2_i S_i (three);
 //   tbar = jet_adj(act, t, ybar_c = f_i Gbar_{k(i),c});  dbias[k] += Gbar_{k,0}.
 // One warp per pair: lanes stride the features of each block, the sums are butterfly-reduced so every lane holds them
-// and runs the (uniform) program itself.  b / bbar are [n][ldb], b2 / b2bar [n][ldb2], t / tbar [C][n][ldt] with plane
-// stride tplane; the adjoint is written only when bbar != NULL (then tbar, and b2bar with b2, too), padding columns
+// and runs the (uniform) program itself.  b / bbar are [n][ldb], b2 / b2bar [n][ldb2], b3 / b3bar [n][ldb3], t / tbar
+// [C][n][ldt] with plane stride tplane; the adjoint is written only when bbar != NULL (then tbar, and b2bar with b2,
+// b3bar with b3, too), padding columns
 // n_out F .. ld-1 of all of them get zeros.  CB bounds the channel count C; the Taylor order bound follows from it.
+// B3: the instance with the third factor (b3 given, then b2 too); the others run the one- and two-factor arithmetic
+// only, so that their register allocation does not pay for the third.
 constexpr int DEEPONET_MAX_OUT = 3;
 constexpr int DEEPONET_MAX_CHANNELS = 7;  // channel bound of the largest head instance
 
@@ -976,9 +982,12 @@ struct DeepONetJetArgs {
   T* b2bar;
   T* tbar;
   T* dbias;  // [n_out] or null
+  const T* b3;  // third branch factor or null (only with b2)
+  int ldb3;
+  T* b3bar;
 };
 
-template <typename T, int CB>
+template <typename T, int CB, bool B3>
 __global__ void __launch_bounds__(256) k_deeponet_jet_head(DeepONetJetArgs<T> h) {
   constexpr int KM = CB - 1 < 4 ? CB - 1 : 4;
   constexpr int NO = DEEPONET_MAX_OUT;
@@ -993,6 +1002,7 @@ __global__ void __launch_bounds__(256) k_deeponet_jet_head(DeepONetJetArgs<T> h)
   for (long long p = (long long)blockIdx.x * wpb + wib; p < h.n; p += (long long)gridDim.x * wpb) {
     const T* bp = h.b + p * h.ldb;
     const T* b2p = h.b2 ? h.b2 + p * h.ldb2 : nullptr;
+    const T* b3p = B3 ? h.b3 + p * h.ldb3 : nullptr;
     const T* tp = h.t + p * h.ldt;
     T G[NO][CB];
 #pragma unroll
@@ -1003,7 +1013,11 @@ __global__ void __launch_bounds__(256) k_deeponet_jet_head(DeepONetJetArgs<T> h)
       for (int i = k * h.F + lane; i < (k + 1) * h.F; i += 32) {
         T y0, s[6];
         act_coef<T, KM>(h.act, tp[i], y0, s);
-        const T fi = b2p ? bp[i] * b2p[i] : bp[i];
+        T fi;
+        if constexpr (B3)
+          fi = bp[i] * b2p[i] * b3p[i];
+        else
+          fi = b2p ? bp[i] * b2p[i] : bp[i];
         G[k][0] += fi * y0;
         jet_fwd<T, DynLay<KM>>(h.J, s, [&](int c) { return tp[(long long)c * h.tplane + i]; }, [&](int c, T v) {
 #pragma unroll
@@ -1049,6 +1063,7 @@ __global__ void __launch_bounds__(256) k_deeponet_jet_head(DeepONetJetArgs<T> h)
     }
     T* bbp = h.bbar + p * h.ldb;
     T* b2bp = h.b2bar ? h.b2bar + p * h.ldb2 : nullptr;
+    T* b3bp = B3 ? h.b3bar + p * h.ldb3 : nullptr;
     T* tbp = h.tbar + p * h.ldt;
 #pragma unroll
     for (int k = 0; k < NO; ++k) {
@@ -1066,7 +1081,13 @@ __global__ void __launch_bounds__(256) k_deeponet_jet_head(DeepONetJetArgs<T> h)
             if (c == q) acc += Gb[k][q] * v;
         });
         T fi = bi;
-        if (b2p) {
+        if constexpr (B3) {
+          const T ci = b2p[i], di = b3p[i];
+          fi = bi * ci * di;
+          b2bp[i] = (bi * di) * acc;
+          b3bp[i] = (bi * ci) * acc;
+          acc = (ci * di) * acc;
+        } else if (b2p) {
           const T ci = b2p[i];
           fi = bi * ci;
           b2bp[i] = bi * acc;
@@ -1084,6 +1105,8 @@ __global__ void __launch_bounds__(256) k_deeponet_jet_head(DeepONetJetArgs<T> h)
       }
     }
     // padding of the row pitches: the sub-networks' adjoints read zeros there
+    if constexpr (B3)
+      for (int i = n_out * h.F + lane; i < h.ldb3; i += 32) b3bp[i] = T(0);
     for (int i = n_out * h.F + lane; i < h.ldb || i < h.ldt || (b2bp && i < h.ldb2); i += 32) {
       if (i < h.ldb) bbp[i] = T(0);
       if (b2bp && i < h.ldb2) b2bp[i] = T(0);

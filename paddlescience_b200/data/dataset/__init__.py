@@ -1,7 +1,8 @@
-from .array_dataset import (ContinuousNamedArrayDataset, DeviceUniformSampler, IterableNamedArrayDataset,
-                            NamedArrayDataset)
+from .array_dataset import (ChipHeatDataset, ContinuousNamedArrayDataset, DeviceUniformSampler,
+                            IterableNamedArrayDataset, NamedArrayDataset)
 
-__all__ = ["NamedArrayDataset", "IterableNamedArrayDataset", "ContinuousNamedArrayDataset", "DeviceUniformSampler", "build_dataset"]
+__all__ = ["NamedArrayDataset", "IterableNamedArrayDataset", "ContinuousNamedArrayDataset", "DeviceUniformSampler", "ChipHeatDataset",
+           "build_dataset"]
 
 
 def build_dataset(cfg):

@@ -150,3 +150,58 @@ class DeviceUniformSampler:
         lib.check(rc, "sample_uniform")
         self.calls += 1
         return dict(zip(self.keys, cols))
+
+
+class ChipHeatDataset:
+    """The chip-heat operator dataset (array_dataset.py:234-312): sample ``idx`` is one cell of the cartesian product of
+    the inputs named in ``index`` (point x source function x boundary type x boundary function), decoded as a
+    mixed-radix number whose first digit varies fastest.  ``y`` follows ``x``'s digit; ``u_one`` (the source or
+    boundary function at that point) is row ``len(input[data_type]) * i_x + i_{data_type}``; every other input key is
+    indexed by its own digit.  Labels and weights are per-constraint constants, repeated for every sample.
+
+    ``idx`` may be one index or an integer array: a batch is gathered in one vectorised pass (what the batch loader
+    asks for), the same rows the reference's per-sample loop would collate."""
+
+    batch_index: bool = True
+
+    def __init__(self, input: Dict[str, np.ndarray], label: Dict[str, np.ndarray], index, data_type: str,
+                 weight: Optional[Dict[str, np.ndarray]] = None, transforms=None):
+        self.input = input
+        self.label = label
+        self.input_keys = tuple(input.keys())
+        self.label_keys = tuple(label.keys())
+        self.index = tuple(index)
+        self.data_type = data_type
+        self.weight = {} if weight is None else weight
+        self.transforms = transforms
+
+    def __getitem__(self, idx):
+        quotient = np.asarray(idx, dtype=np.int64)
+        digit = {}
+        for k in dict.fromkeys(self.index):
+            num = len(self.input[k])
+            digit[k] = quotient % num
+            quotient = quotient // num
+        input_item = {}
+        for key, v in self.input.items():
+            if key == "y":
+                input_item[key] = v[digit["x"]]
+            elif key == "u_one":
+                input_item[key] = v[len(self.input[self.data_type]) * digit["x"] + digit[self.data_type]]
+            else:
+                input_item[key] = v[digit[key]]
+        if np.ndim(idx) == 0:
+            label_item, weight_item = dict(self.label), dict(self.weight)
+        else:
+            n = len(idx)
+            label_item = {k: np.repeat(np.asarray(v)[None], n, axis=0) for k, v in self.label.items()}
+            weight_item = {k: np.repeat(np.asarray(v)[None], n, axis=0) for k, v in self.weight.items()}
+        if self.transforms is not None:
+            input_item, label_item, weight_item = self.transforms((input_item, label_item, weight_item))
+        return input_item, label_item, weight_item
+
+    def __len__(self):
+        n = 1
+        for k in self.index:
+            n *= len(self.input[k])
+        return n

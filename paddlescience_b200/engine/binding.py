@@ -45,6 +45,7 @@ OPS = {
     "const": 0, "mov": 1, "add": 2, "sub": 3, "mul": 4, "div": 5, "neg": 6, "powi": 7, "pow": 8,
     "sin": 9, "cos": 10, "tanh": 11, "exp": 12, "log": 13, "sqrt": 14, "abs": 15, "max": 16,
     "min": 17, "sign": 18, "fma": 19, "sinh": 20, "cosh": 21, "heaviside": 22,
+    "eq": 23, "select": 24,
 }
 
 REDUCE_MEAN, REDUCE_SUM = 0, 1
@@ -147,6 +148,9 @@ class DeepONetJetArgs(C.Structure):
         ("b2bar", C.c_void_p),
         ("tbar", C.c_void_p),
         ("dbias", C.c_void_p),
+        ("b3", C.c_void_p),
+        ("ldb3", C.c_int32),
+        ("b3bar", C.c_void_p),
     ]
 
 

@@ -11,6 +11,11 @@ ppsci/utils/symbolic.py:681-981).  The reference turns a sympy tree into a list 
 * a straight-line register program evaluating all residuals r_k AND all partials
   d r_k / d (output-jet channel) — so the adjoint needs no autograd graph.  ``detach(...)``
   sub-expressions (ppsci/equation/pde/base.py:91-151) contribute values but no partials.
+
+``Piecewise`` (``torch.where(cond, a, b)`` / ``paddle.where`` in a traced expression) lowers to EQ + SELECT: a true
+select, so a NaN or Inf of an untaken branch never reaches the residual or its partials.  Conditions must be
+equalities ``a == b`` (the last branch's ``True`` aside); the partials differentiate each branch, the conditions
+contribute none.
 """
 from __future__ import annotations
 
@@ -380,6 +385,27 @@ class _Emitter:
                 self.release(r, o)
                 acc, own = dst, True
             return acc, own
+        if isinstance(e, sp.Eq):
+            ra, oa = self.emit(e.lhs)
+            rb, ob = self.emit(e.rhs)
+            dst = self._dst(ra, oa)
+            self.op("eq", dst, ra, rb)
+            self.release(rb, ob)
+            return dst, True
+        if isinstance(e, (sp.Or, sp.And)):
+            # on 0 / 1 values max is "or" and min is "and"; sympy forms these when differentiating a Piecewise merges
+            # neighbouring branches with equal partials
+            name = "max" if isinstance(e, sp.Or) else "min"
+            acc, own = self.emit(e.args[0])
+            for t in e.args[1:]:
+                r, o = self.emit(t)
+                dst = self._dst(acc, own)
+                self.op(name, dst, acc, r)
+                self.release(r, o)
+                acc, own = dst, True
+            return acc, own
+        if isinstance(e, sp.Piecewise):
+            return self._select(list(e.args))
         if isinstance(e, sp.tan):
             rs, os_ = self.emit(sp.sin(e.args[0]))
             rc, oc = self.emit(sp.cos(e.args[0]))
@@ -390,6 +416,38 @@ class _Emitter:
         raise NotImplementedError(
             f"The node {e} (type {type(e).__name__}) is not supported in the residual program."
         )
+
+
+    def _select(self, pieces) -> Tuple[int, bool]:
+        """Piecewise((v_0, c_0), (v_1, c_1), ..., (v_n, True)) as nested SELECTs: the condition's 0 / 1 in dst, then
+        dst = dst != 0 ? v_0 : (the rest)."""
+        (val, cond), rest = pieces[0], pieces[1:]
+        if cond == sp.true:
+            return self.emit(val)
+        rc, oc = self.emit(cond)
+        dst = self._dst(rc, oc)
+        if dst != rc:
+            self.op("mov", dst, rc)
+        ra, oa = self.emit(val)
+        rb, ob = self._select(rest)
+        self.op("select", dst, ra, rb)
+        self.release(ra, oa)
+        self.release(rb, ob)
+        return dst, True
+
+
+def _check_piecewise(name: str, e: sp.Basic):
+    """Only ``where(a == b, x, y)`` chains: every condition an equality, the last one ``True``."""
+    for pw in e.atoms(sp.Piecewise):
+        conds = [c for _, c in pw.args]
+        for c in conds[:-1]:
+            if not isinstance(c, sp.Eq):
+                raise NotImplementedError(
+                    f"residual '{name}': the condition {c} of a piecewise expression is not supported; conditions must be "
+                    "equalities, as in torch.where(x == c, a, b) (nested for more cases)")
+        if conds[-1] != sp.true:
+            raise NotImplementedError(f"residual '{name}': a piecewise expression needs a final default branch "
+                                      "(torch.where(x == c, a, b) always has one)")
 
 
 def _is_detach(e: sp.Basic) -> bool:
@@ -422,6 +480,8 @@ def compile_residuals(
 
     names = list(exprs.keys())
     raw = [sp.sympify(exprs[n]) for n in names]
+    for n, e in zip(names, raw):
+        _check_piecewise(n, e)
 
     # ---- 1. collect derivative multi-indices ------------------------------------------------
     alphas = set()
@@ -555,6 +615,20 @@ def compile_residuals(
     # ---- 4. CSE + emission -------------------------------------------------------------------
     n_fixed = C * n_out + n_in + len(aux_list)
     all_exprs = values + [g for _, _, g in grads] + [g for _, _, g in pgrads]
+    # every Piecewise is emitted whole, ahead of CSE, into a register live to the end: CSE never sees inside a branch,
+    # so no part of a branch is computed outside its select
+    pw_sym: Dict[sp.Piecewise, sp.Symbol] = {}
+
+    def hide_piecewise(e: sp.Basic) -> sp.Basic:
+        if isinstance(e, sp.Piecewise):
+            if e not in pw_sym:
+                pw_sym[e] = sp.Symbol(f"PW_{len(pw_sym)}", real=True)
+            return pw_sym[e]
+        if not e.args:
+            return e
+        return e.func(*[hide_piecewise(a) for a in e.args])
+
+    all_exprs = [hide_piecewise(e) for e in all_exprs]
     repl, reduced = sp.cse(all_exprs, order="none") if all_exprs else ([], [])
     em = _Emitter(n_fixed)
     for (c, j), s in ysym.items():
@@ -563,6 +637,9 @@ def compile_residuals(
         em.sym_reg[s] = C * n_out + i
     for nm, s in auxsym.items():
         em.sym_reg[s] = C * n_out + n_in + aux_list.index(nm)
+    for pw, s in pw_sym.items():
+        r, owned = em.emit(pw)  # a Piecewise register is always owned (its select's dst)
+        em.sym_reg[s] = r
     # liveness of CSE temporaries
     stmts = [e for _, e in repl] + list(reduced)
     last_use: Dict[sp.Symbol, int] = {}
