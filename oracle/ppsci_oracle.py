@@ -302,6 +302,9 @@ def eval_expr(expr: sp.Basic, data: Dict[str, torch.Tensor]) -> torch.Tensor:
         for cls, fn in table.items():
             if isinstance(e, cls):
                 return fn(ev(e.args[0]))
+        if isinstance(e, sp.Heaviside):  # a step: zero gradient, as paddle.heaviside
+            a = ev(e.args[0]).detach()
+            return torch.heaviside(a, torch.full_like(a, float(e.args[1]) if len(e.args) > 1 else 0.5))
         if isinstance(e, sp.Max):
             acc = ev(e.args[0])
             for a in e.args[1:]:

@@ -365,9 +365,11 @@ class _Emitter:
             self.op("pow", dst, rb, re_)
             self.release(re_, oe)
             return dst, True
+        if isinstance(e, sp.Heaviside):
+            return self._heaviside(e)
         unary = {
             sp.sin: "sin", sp.cos: "cos", sp.tanh: "tanh", sp.exp: "exp", sp.log: "log",
-            sp.Abs: "abs", sp.sign: "sign", sp.sinh: "sinh", sp.cosh: "cosh", sp.Heaviside: "heaviside",
+            sp.Abs: "abs", sp.sign: "sign", sp.sinh: "sinh", sp.cosh: "cosh",
         }
         for cls, name in unary.items():
             if isinstance(e, cls):
@@ -417,6 +419,28 @@ class _Emitter:
             f"The node {e} (type {type(e).__name__}) is not supported in the residual program."
         )
 
+
+    def _heaviside(self, e: sp.Heaviside) -> Tuple[int, bool]:
+        """Heaviside(a, H0): the HEAVISIDE op gives 1/2 at a == 0; any other constant H0 is selected there."""
+        h0 = e.args[1] if len(e.args) > 1 else sp.S.Half
+        if not h0.is_Number:
+            raise NotImplementedError(f"{e}: the value at zero H0 = {h0} of a Heaviside step must be a constant")
+        ra, oa = self.emit(e.args[0])
+        if h0 == sp.S.Half:
+            dst = self._dst(ra, oa)
+            self.op("heaviside", dst, ra)
+            return dst, True
+        rz = self.const(0.0)
+        rc = self.alloc()
+        self.op("eq", rc, ra, rz)  # the select's condition: a == 0
+        self.release(rz, True)
+        rh = self.const(float(h0))
+        rv = self._dst(ra, oa)
+        self.op("heaviside", rv, ra)
+        self.op("select", rc, rh, rv)
+        self.release(rh, True)
+        self.release(rv, True)
+        return rc, True
 
     def _select(self, pieces) -> Tuple[int, bool]:
         """Piecewise((v_0, c_0), (v_1, c_1), ..., (v_n, True)) as nested SELECTs: the condition's 0 / 1 in dst, then
@@ -590,13 +614,17 @@ def compile_residuals(
             e = e.xreplace({s: det_subs[s] for s in syms})
         return e
 
+    def partial(e: sp.Basic, s: sp.Symbol) -> sp.Basic:
+        # the partials of sign and Heaviside are DiracDelta terms: zero almost everywhere, and zero in autograd
+        return sp.diff(e, s).replace(lambda z: isinstance(z, sp.DiracDelta), lambda z: sp.S.Zero)
+
     values = [restore(e) for e in stripped]
     grads: List[Tuple[int, int, sp.Basic]] = []  # (res k, input reg idx, expr)
     if with_grad:
         for k, e in enumerate(stripped):
             for (c, j), s in sorted(ysym.items()):
                 if s in e.free_symbols:
-                    g = sp.diff(e, s)
+                    g = partial(e, s)
                     if g != 0:
                         grads.append((k, c * n_out + j, restore(g)))
     grads.sort(key=lambda t: (t[1], t[0]))
@@ -606,7 +634,7 @@ def compile_residuals(
         for k, e in enumerate(stripped):
             for nm, s_ in auxsym.items():
                 if nm in param_set and s_ in e.free_symbols:
-                    g = sp.diff(e, s_)
+                    g = partial(e, s_)
                     if g != 0:
                         pgrads.append((k, aux_list.index(nm), restore(g)))
     if len(pgrads) > B.MAX_PGRAD:
