@@ -253,8 +253,15 @@ int64_t ppsci_b200_plan_last_launches(const ppsci_plan* plan);
  * layer == 301 / 302: the two ping-pong buffers of the hidden adjoints Zbar.  After an adjoint over L = n_layers
  * layers, Zbar_l (l >= 1) was last written to buffer (L-1-l) mod 2 (301 for 0, 302 for 1), so only the two lowest,
  * Zbar_1 and Zbar_2, survive the call.  Zbar_l is laid out [C][min(n_points, chunk)][round4(width_l)], plane pitch
- * min(n_points, chunk) * round4(width_l).  After a multi-chunk call every buffer holds the last chunk.  The rule does
- * not hold for gated networks (ModifiedMLP, PirateNet), whose gate kernels also work in these buffers. */
+ * min(n_points, chunk) * round4(width_l).  After a multi-chunk call every buffer holds the last chunk.  In gated
+ * networks (ModifiedMLP, PirateNet) the dx GEMM writes the adjoint of G_l there and the gate or mix kernel turns it
+ * into Zbar_l in place, so the same holds.
+ * Gated plans: 400 + l -> G_l (l in [1, n_layers)), the stored output of the gate or mix after hidden layer l;
+ * 310 / 311 -> the embeddings' pre-activations Zu / Zv, 312 / 313 -> their adjoints Zubar / Zvbar (width of the first
+ * gated layer); 314 -> Xres, the adjoint carried by PirateNet's residual path (layer 1's width).
+ * 500 + l: Zbar_l of hidden layer l in a plane set of its own, when the plan was created with the environment variable
+ * PPSCI_B200_KEEP_ADJOINTS set (every Zbar_l then survives the call; the kernels and launches are unchanged).
+ * Returns -1 for a code whose buffer the plan does not carve. */
 int64_t ppsci_b200_plan_stash_offset(const ppsci_plan* plan, int64_t n_points, int32_t layer);
 
 /* Forward + adjoint of the network VALUES for caller-supplied output adjoints: runs the forward pass (stash), seeds

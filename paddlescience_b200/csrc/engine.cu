@@ -80,6 +80,9 @@ struct ppsci_plan {
   bool thin_first = false;
   bool thin_last = false;
   bool thin_vec = false;
+  // PPSCI_B200_KEEP_ADJOINTS (tests): every hidden layer's Zbar gets a plane set of its own instead of the two ping-pong
+  // sets, so that all of them survive a call; kernels and launches are the same
+  bool keep_adj = false;
   // device copies of the residual program
   int* d_prog = nullptr;
   double* d_consts = nullptr;
@@ -135,6 +138,7 @@ struct Carve {
   size_t zu, zv, zub, zvb;
   size_t xres, wtu, wtv;  // gated == 2: adjoint carried by the blocks' residual path; transposed embedding weights
   size_t omega_acc;       // fp64 dLoss/d omega accumulators of a call (n_omega)
+  size_t zbl[PPSCI_MAX_LAYERS + 1];  // keep_adj: Zbar_l of hidden layer l (empty otherwise)
   size_t total;
 };
 
@@ -175,6 +179,7 @@ static void carve(const ppsci_plan* P, int64_t nc, Carve* cv) {
   cv->wtu = take(gated && emb ? (size_t)P->spec.widths[1] * P->spec.widths[lg] * es : 0);
   cv->wtv = take(gated && emb ? (size_t)P->spec.widths[1] * P->spec.widths[lg] * es : 0);
   cv->omega_acc = take((size_t)P->spec.n_omega * sizeof(double));
+  for (int l = 1; l < L; ++l) cv->zbl[l] = take(P->keep_adj ? (size_t)P->C * nc * P->ld[l] * es : 0);
   cv->total = off;
 }
 
@@ -414,6 +419,7 @@ extern "C" int ppsci_b200_plan_create(const ppsci_plan_spec* s, ppsci_plan** out
   P->thin_first = thin_on && s->n_layers >= 2 && s->widths[0] <= THIN_MAXF && !s->dense_in && !s->gated;
   P->thin_last = thin_on && s->n_layers >= 2 && n_out <= THIN_MAXM && C * n_out <= THIN_MAXCM && !s->gated && !act_has_param(s->act);
   P->thin_vec = s->dtype == PPSCI_F32 && with_lay(ThinLays{}, P->J, [](auto) {}) && getenv("PPSCI_B200_NO_THINV") == nullptr;
+  P->keep_adj = getenv("PPSCI_B200_KEEP_ADJOINTS") != nullptr;
   if (s->backend == 2 && !P->use_wg) {
     delete P;
     return fail("plan_create: backend=2 (tensor cores) requested but the plan is not eligible (needs f32, hidden widths that "
@@ -489,16 +495,26 @@ extern "C" int32_t ppsci_b200_plan_uses_tcgen05(const ppsci_plan* P) { return (P
 // `layer` for a call with n_points points: layer in [1, n_layers) -> hidden pre-activations Z_l,
 // layer == n_layers -> output jets Y.  Layout [C][min(n_points, chunk)][ld], ld = round4(width).
 // 301 / 302 -> the Zbar ping-pong buffers zbar0 / zbar1 (the adjoint writes Zbar_l into buffer (L-1-l) mod 2).
+// Gated plans: 400 + l -> G_l, the stored output of the gate or mix after hidden layer l; 310 / 311 -> Zu / Zv,
+// 312 / 313 -> their adjoints Zubar / Zvbar (width of the first gated layer); 314 -> Xres (PirateNet, layer 1's width).
+// 500 + l -> Zbar_l of hidden layer l when the plan was created with PPSCI_B200_KEEP_ADJOINTS set.
+// -1 for a code whose buffer the plan does not carve.
 extern "C" int64_t ppsci_b200_plan_stash_offset(const ppsci_plan* P, int64_t n_points, int32_t layer) {
   if (!P || n_points <= 0) return -1;
   const int64_t nc = n_points < P->chunk ? n_points : P->chunk;
   Carve cv;
   carve(P, nc, &cv);
+  const int L = P->spec.n_layers;
+  const bool gated = P->spec.gated != 0;
   if (layer == 300) return (int64_t)cv.ybar;  // output adjoints Ybar (values_bwd_kept accepts this address: no seeding copy)
   if (layer == 301) return (int64_t)cv.zbar0;
   if (layer == 302) return (int64_t)cv.zbar1;
-  if (layer < 1 || layer > P->spec.n_layers) return -1;
-  return (int64_t)(layer < P->spec.n_layers ? cv.z[layer] : cv.y);
+  if (layer >= 310 && layer <= 313) return gated ? (int64_t)(layer == 310 ? cv.zu : layer == 311 ? cv.zv : layer == 312 ? cv.zub : cv.zvb) : -1;
+  if (layer == 314) return P->spec.gated == 2 ? (int64_t)cv.xres : -1;
+  if (layer > 400 && layer < 400 + L) return gated ? (int64_t)cv.gt[layer - 400] : -1;
+  if (layer > 500 && layer < 500 + L) return P->keep_adj ? (int64_t)cv.zbl[layer - 500] : -1;
+  if (layer < 1 || layer > L) return -1;
+  return (int64_t)(layer < L ? cv.z[layer] : cv.y);
 }
 
 extern "C" size_t ppsci_b200_plan_workspace_bytes(const ppsci_plan* P, int64_t n_points) {
@@ -628,8 +644,11 @@ static int run(ppsci_plan* P, const CallArgs& a) {
     PPSCI_LAUNCH(kernel, grid, block, smem, st, args...);
     P->launches++;
   };
-  // Zbar_l: Ybar for l == L, otherwise ping-pong buffer (L - 1 - l) mod 2 (include/ppsci_b200.h)
-  auto zbar = [&](int l) { return reinterpret_cast<T*>(ws + (l == L ? cv.ybar : (L - 1 - l) % 2 ? cv.zbar1 : cv.zbar0)); };
+  // Zbar_l: Ybar for l == L, otherwise ping-pong buffer (L - 1 - l) mod 2 (include/ppsci_b200.h), or with keep_adj
+  // a plane set of its own
+  auto zbar = [&](int l) {
+    return reinterpret_cast<T*>(ws + (l == L ? cv.ybar : P->keep_adj ? cv.zbl[l] : (L - 1 - l) % 2 ? cv.zbar1 : cv.zbar0));
+  };
   const int TP = TM / C;
   const int PT = RC / C;
   const bool gated = s.gated != 0;  // ModifiedMLP: generic tile GEMMs + the gate kernels (kernels_gate.cuh)

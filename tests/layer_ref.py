@@ -47,12 +47,14 @@ def last_chunk(plan, n: int) -> Tuple[int, int]:
     return x_off, n - x_off
 
 
-def stash_views(plan, n: int, last: bool = False) -> Dict[str, torch.Tensor]:
+def stash_views(plan, n: int, last: bool = False,
+                extra: Optional[Dict[str, Tuple[int, int]]] = None) -> Dict[str, torch.Tensor]:
     """Views [C, n, width] into ``plan``'s workspace after its most recent call, which took ``n`` points:
     "Z<l>" for every hidden layer, "Y", "Ybar", and "Zbar1" / "Zbar2" for the hidden adjoints that survive the call
     (Zbar_l was last written to buffer (L-1-l) mod 2).  Needs n <= plan.chunk_points (one workspace chunk), unless
     ``last``: then the views cover the points of the call's last chunk (``last_chunk``), which the workspace still
-    holds; their weight gradients are sums over every chunk and cannot be checked from them."""
+    holds; their weight gradients are sums over every chunk and cannot be checked from them.  ``extra``: {name:
+    (stash code, width)} of more planes to view."""
     if n > plan.chunk_points and not last:
         raise ValueError(f"{n} points span more than one workspace chunk ({plan.chunk_points} points)")
     n_pts = last_chunk(plan, n)[1] if last else n
@@ -79,6 +81,8 @@ def stash_views(plan, n: int, last: bool = False) -> Dict[str, torch.Tensor]:
     for l in (1, 2):
         if l < L:
             out[f"Zbar{l}"] = view(CODE_ZBAR0 + (L - 1 - l) % 2, widths[l])
+    for name, (code, width) in (extra or {}).items():
+        out[name] = view(code, width)
     return out
 
 
@@ -391,22 +395,26 @@ def check_layer(plan, views: Dict[str, torch.Tensor], params: torch.Tensor, grad
 
 
 def omega_errors(plan, views: Dict[str, torch.Tensor], params: torch.Tensor, grads: torch.Tensor,
-                 seed: Optional[torch.Tensor] = None) -> float:
+                 seed: Optional[torch.Tensor] = None,
+                 consumers: Optional[Sequence[Tuple[torch.Tensor, torch.Tensor]]] = None) -> float:
     """dLoss/d omega of the trainable frequencies against fp64 autograd through omega of ``seed_jets``, contracted
     with the engine's Zbar_1 W_1^T:  sum_{c,p,f} d seed_c[p][f] / d omega_j  (Zbar_1 W_1^T)[c][p][f].  Componentwise:
-    the error over the same contraction on absolute values (``dseed_abs`` |Zbar_1| |W_1|^T) plus |seed|."""
+    the error over the same contraction on absolute values (``dseed_abs`` |Zbar_1| |W_1|^T) plus |seed|.
+    ``consumers``: the (Zbar, W) pairs of every GEMM that read the seeds, when there are more than layer 1's."""
     net = plan.compiled.net
-    w_sl, _, (K, N) = param_blocks(net.widths)[0]
-    W = params[w_sl].view(K, N).double()
-    zb = views["Zbar1"].double()
+    if consumers is None:
+        w_sl, _, (K, N) = param_blocks(net.widths)[0]
+        consumers = [(views["Zbar1"], params[w_sl].view(K, N))]
     om_f = feature_omegas(plan, params).detach()
     idx = net.feat_omega_param
     o0 = omega_offset(net)
     om = params[o0: o0 + net.n_omega].double().detach().requires_grad_(True)
     om_feat = torch.stack([om[j] if j >= 0 else om_f[f] for f, j in enumerate(idx)])
     A = seed_jets(plan.compiled, views["X"], om_feat)
-    (ref,) = torch.autograd.grad((A * (zb @ W.T)).sum(), om)
-    per_feat = (dseed_abs(plan.compiled, views["X"], om_f) * (zb.abs() @ W.abs().T)).sum((0, 1))
+    D = sum(zb.double() @ W.double().T for zb, W in consumers)
+    Da = sum(zb.double().abs() @ W.double().abs().T for zb, W in consumers)
+    (ref,) = torch.autograd.grad((A * D).sum(), om)
+    per_feat = (dseed_abs(plan.compiled, views["X"], om_f) * Da).sum((0, 1))
     bound = torch.zeros_like(ref)
     for f, j in enumerate(idx):
         if j >= 0:
