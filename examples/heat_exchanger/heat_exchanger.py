@@ -9,8 +9,8 @@ head; x and t derivatives come from the trunk's Taylor jets.
 
 The grid is the one ``TimeXGeometry(TimeDomain(0, 1, timestamps=linspace(0, 2, NTIME + 1)), Interval(0, DL))
 .sample_interior(NPOINT * NTIME, evenly=True)`` gives (ppsci/geometry/timedomain.py:156-201), built here with numpy:
-time-major, t = timestamps[1:], and for each t, x = linspace(0, DL, NPOINT).  ``TimeXGeometry`` itself is not part of
-this package.  The grid is replicated over NQM x NQM random (qm_h, qm_c) pairs the way the reference does.
+time-major, t = timestamps[1:], and for each t, x = linspace(0, DL, NPOINT) (``geometry.TimeXGeometry`` gives the same
+points, tests/test_time_geometry.py).  The grid is replicated over NQM x NQM random (qm_h, qm_c) pairs the way the reference does.
 
 Besides the reference's validators (MSE of the boundary conditions and the residuals on a held-out (qm_h, qm_c)),
 ``main`` checks the trained operator against an independent solution the reference does not have: an upwind

@@ -227,8 +227,12 @@ __global__ void __launch_bounds__(256) k_last_fwd_v(LastArgs<float> g) {
 }
 
 // Output layer backward, fused (see k_last_bwd).  Block = 64 k quads x 4 point lanes; grid (ceil(K/256), point blocks).
+// Lay122 declares one resident block per SM: without it ptxas spills 12 bytes around the reciprocal's slow-path call at
+// M = 2 (80 registers).  0 leaves the other layouts' launch bounds, and their code, as they were.
+template <class L>
+constexpr int last_bwd_min_blocks = std::is_same<L, Lay122>::value ? 1 : 0;
 template <class L, int M>
-__global__ void __launch_bounds__(256) k_last_bwd_v(LastArgs<float> g) {
+__global__ void __launch_bounds__(256, last_bwd_min_blocks<L>) k_last_bwd_v(LastArgs<float> g) {
   constexpr int CS = L::CS;
   __shared__ float red[3][64][4 * M];
   const int tid = threadIdx.x;

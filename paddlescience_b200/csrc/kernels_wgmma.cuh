@@ -436,7 +436,7 @@ __host__ __device__ constexpr int dw_ksteps(int C) { return (dw_groups(C) + 1) /
 __host__ __device__ constexpr int dw_atoms(int C) { return (dw_ksteps(C) + 3) / 4; }  // 32-wide K atoms per B stage
 // widest column block in units of 32: two accumulators of BN / 2 registers each, beside the A fragments and the B
 // prefetch of a chunk, must fit in 255 registers without spilling
-__host__ __device__ constexpr int dw_maxq(int C) { return C <= 5 ? 4 : C <= 8 ? 2 : 1; }
+__host__ __device__ constexpr int dw_maxq(int C) { return C <= 6 ? 4 : C <= 8 ? 2 : 1; }
 // two stages of [hi | lo][atoms][BN rows x 128 bytes], 1024-byte aligned, then the db_l column sums, the A operand's
 // per-thread Z_{l-1} slots and the per-thread partial sums of the flushed accumulators (BN / 2 per thread)
 __host__ __device__ constexpr int dw_smem_bytes(int C, int bnq) {

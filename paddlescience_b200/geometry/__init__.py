@@ -3,8 +3,9 @@ from .geometry_1d import Interval
 from .geometry_2d import Rectangle
 from .geometry_3d import Cuboid
 from .geometry_nd import Hypercube
+from .timedomain import TimeDomain, TimeXGeometry
 
-__all__ = ["Geometry", "Interval", "Rectangle", "Cuboid", "Hypercube", "build_geometry"]
+__all__ = ["Geometry", "Interval", "Rectangle", "Cuboid", "Hypercube", "TimeDomain", "TimeXGeometry", "build_geometry"]
 
 
 def build_geometry(cfg):

@@ -12,8 +12,10 @@ from . import base
 
 
 class GeometryValidator(base.Validator):
-    """Same arguments as the reference (geo_validator.py:72-85).  Time-dependent geometries (``TimeXGeometry``) are
-    not part of this package yet and raise ``NotImplementedError``."""
+    """Same arguments as the reference (geo_validator.py:72-85).  On a ``TimeXGeometry`` with timestamps (or a time
+    step), ``total_size`` is split evenly over the times: the points after t0, time-major, and with ``with_initial``
+    also ``total_size / num_timestamps`` points at t0 in front of them (geo_validator.py:94-130).  Random times
+    raise ``NotImplementedError``, as in the reference."""
 
     def __init__(
         self,
@@ -33,11 +35,22 @@ class GeometryValidator(base.Validator):
         self.label_dict = label_dict
         self.input_keys = geom.dim_keys
         self.output_keys = tuple(label_dict.keys())
-        if hasattr(geom, "timedomain"):
-            raise NotImplementedError("GeometryValidator on a TimeXGeometry is not implemented yet.")
         self.num_timestamps = 1
         nx = dataloader_cfg["total_size"]
-        inputs = geom.sample_interior(nx, random, criteria, evenly)
+        if hasattr(geom, "timedomain"):
+            nts = geom.timedomain.num_timestamps
+            if nts is None:
+                raise NotImplementedError("TimeXGeometry with random timestamp not implemented yet.")
+            self.num_timestamps = nts if with_initial else nts - 1
+            if nx % self.num_timestamps != 0:
+                raise ValueError(f"total_size {nx} is not a multiple of the {self.num_timestamps} timestamps")
+            nx //= self.num_timestamps
+            inputs = geom.sample_interior(nx * (nts - 1), random, criteria, evenly)
+            if with_initial:
+                initial = geom.sample_initial_interior(nx, random, criteria, evenly)
+                inputs = {key: np.vstack((initial[key], inputs[key])) for key in inputs}
+        else:
+            inputs = geom.sample_interior(nx, random, criteria, evenly)
         like = next(iter(inputs.values()))
         label = cbase.materialize(label_dict, inputs, geom.dim_keys, like)
         weight = {key: np.ones_like(next(iter(label.values()))) for key in label}

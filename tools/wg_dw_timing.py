@@ -37,7 +37,7 @@ def dw_pch(C: int) -> int:
 
 
 def dw_maxq(C: int) -> int:
-    return 4 if C <= 5 else 2 if C <= 8 else 1
+    return 4 if C <= 6 else 2 if C <= 8 else 1
 
 
 def _gpu_info() -> dict:
