@@ -49,20 +49,24 @@ struct SLay {
 };
 
 // The compile-time layouts of the kernels: Navier-Stokes / Poisson in 2-D (Lay22) and 3-D (Lay222), a first-order time
-// and a second-order space direction (Lay12), unsteady Navier-Stokes in 2-D on (t, x, y) (Lay122), values only (LayV),
-// and the polarised biharmonic operator (Lay4444).
+// and a second-order space direction (Lay12), unsteady Navier-Stokes in 2-D on (t, x, y) (Lay122) and in 3-D on
+// (x, y, z, t) (Lay2221) or (t, x, y, z) (Lay1222), values only (LayV), and the polarised biharmonic operator (Lay4444).
 using Lay22 = SLay<2, 2, 0, 0>;
 using Lay12 = SLay<1, 2, 0, 0>;
 using Lay222 = SLay<2, 2, 2, 0>;
 using Lay122 = SLay<1, 2, 2, 0>;
+using Lay2221 = SLay<2, 2, 2, 1>;
+using Lay1222 = SLay<1, 2, 2, 2>;
 using LayV = SLay<0, 0, 0, 0>;
 using Lay4444 = SLay<4, 4, 4, 4>;
 
-// The layouts each kernel family is instantiated for; with_lay picks among them.
+// The layouts each kernel family is instantiated for; with_lay picks among them.  Lay1222 is a tensor-core layout only:
+// plans on t:1, x:2, y:2, z:2 (e.g. a heat equation on (t, x, y, z)) have always taken the generic thin first / last
+// layer kernels, and keep them.
 template <class... Ls>
 struct LayList {};
-using ThinLays = LayList<Lay22, Lay12, Lay222, Lay122, LayV>;           // kernels_thin.cuh
-using WgLays = LayList<Lay22, Lay12, Lay222, Lay122, LayV, Lay4444>;    // kernels_wgmma.cuh
+using ThinLays = LayList<Lay22, Lay12, Lay222, Lay122, Lay2221, LayV>;           // kernels_thin.cuh
+using WgLays = LayList<Lay22, Lay12, Lay222, Lay122, Lay2221, Lay1222, LayV, Lay4444>;    // kernels_wgmma.cuh
 
 // f(L{}) for the layout L of the list that J matches; false if none does
 template <class... Ls, class F>

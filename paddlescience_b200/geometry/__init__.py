@@ -3,9 +3,10 @@ from .geometry_1d import Interval
 from .geometry_2d import Rectangle
 from .geometry_3d import Cuboid
 from .geometry_nd import Hypercube
+from .pointcloud import PointCloud
 from .timedomain import TimeDomain, TimeXGeometry
 
-__all__ = ["Geometry", "Interval", "Rectangle", "Cuboid", "Hypercube", "TimeDomain", "TimeXGeometry", "build_geometry"]
+__all__ = ["Geometry", "Interval", "Rectangle", "Cuboid", "Hypercube", "PointCloud", "TimeDomain", "TimeXGeometry", "build_geometry"]
 
 
 def build_geometry(cfg):
